@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- DEFLATE level-6 compress + inflate throughput (GB/s of uncompressed bytes) on B200.
+"""bench.py -- DEFLATE level-6 compress + inflate throughput (GB/s of uncompressed bytes) on the GPU.
 
 One "step" = one pass of the hot path over one batch of synthetic input:
     deflate leg : config C3 -- raw Deflater level 6 on 1024 x 256 KiB Silesia-mix buffers
@@ -32,7 +32,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np  # noqa: E402
 
-METRIC = "DEFLATE level-6 compress + inflate GB/s (uncompressed) at 1/2/4/8 B200 vs C# ref"
+METRIC = "DEFLATE level-6 compress + inflate GB/s (uncompressed) at 1/2/4/8 GPUs vs C# ref"
 N_DEFLATE, SZ_DEFLATE = 1024, 262144      # C3
 N_INFLATE, SZ_INFLATE = 256, 1 << 20       # C2
 
@@ -63,9 +63,10 @@ def make_inputs(rank, n_def, n_inf, workers):
 
 
 class ClockSampler:
-    """samples nvidia-smi clocks / throttle reasons while the timed region runs (B200_PROFILING.md recipe)"""
+    """samples nvidia-smi clocks / throttle reasons while the timed region runs, and the card's name and power limit (a number
+    measured here is only meaningful with both)"""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -93,7 +94,7 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, reasons, card = [], [], set(), {}
         for r in self.rows:
             f = [x.strip() for x in r.split(",")]
             if len(f) < 9:
@@ -103,12 +104,14 @@ class ClockSampler:
                 mx.append(float(f[2]))
             except ValueError:
                 continue
+            if len(f) >= 11:
+                card = {"name": f[10], "power_limit_w": f[9]}
             names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
             for nm, v in zip(names, f[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "reasons": sorted(reasons), "samples": len(sm), **card}
 
 
 def host_threads():
@@ -139,18 +142,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def captured_traffic(kernel, small):
-    """dram bytes (read + write) of one launch of `kernel` on this workload, from the committed ncu --set full capture"""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if small or not os.path.exists(p):
-        return None, None
-    j = json.load(open(p))
-    if j.get("kernel") != kernel:
-        return None, None
-    return int(j["dram_bytes_per_launch"]), j.get("source")
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 INFLATE_KERNELS = ("k_wrap", "k_find", "k_find3", "k_seglist", "k_dec1", "k_chain", "k_dec2", "k_resolve", "k_inflate")
@@ -188,9 +180,8 @@ def workload_name(n_def, n_inf):
 
 def run_reference(args, rank, world, out):
     """--impl reference: the reference's CPU algorithm on all host threads, on the GPU arm's own step: the same generators,
-    the same 1024 + 256 buffers, the same 1:1 mix of the legs, whatever the thread count.  The C# original cannot run here:
-    neither this image nor the GPU boxes have a .NET / mono runtime (profiles/r02_probe_gpu_box.txt; probed again below), so
-    the arm is the line-faithful C++ restatement under oracle/ (kind "port")."""
+    the same 1024 + 256 buffers, the same 1:1 mix of the legs, whatever the thread count.  The C# original needs a .NET / mono
+    runtime (probed below); without one the arm is the line-faithful C++ restatement under oracle/ (kind "port")."""
     if rank != 0:
         return
     import oracle_lib as O
@@ -255,6 +246,35 @@ def _max_over_ranks(dist, world, ms, dev):
     return ms
 
 
+DUMP_SAMPLE_DEFLATE, DUMP_SAMPLE_INFLATE, DUMP_LIMIT = 32, 4, 64 << 20
+
+
+def dump_outputs(path, d_off, d_out, d_len, d_st, i_off, i_out, i_len, i_st, i_used):
+    """--dump-outputs: what a caller of the timed step receives, per leg -- every stream's length, status and CRC-32 of its
+    bytes (inflate: and the input bytes it consumed), and the bytes themselves of a fixed, seeded sample of streams
+    (<= DUMP_LIMIT in all).  Byte values and uint32 CRCs are exact in float32 / float64, so two builds compare exactly."""
+    import zlib
+    os.makedirs(path, exist_ok=True)
+    arrays = {}
+    for leg, off, buf, ln, st, nsample in (("deflate", d_off, d_out, d_len, d_st, DUMP_SAMPLE_DEFLATE),
+                                           ("inflate", i_off, i_out, i_len, i_st, DUMP_SAMPLE_INFLATE)):
+        lens = ln.cpu().numpy().astype(np.int64)
+        host = buf.cpu().numpy()
+        streams = [host[int(o):int(o) + int(n)] for o, n in zip(off, lens)]
+        pick = np.sort(np.random.default_rng(20261015).choice(len(streams), min(nsample, len(streams)), replace=False))
+        arrays[leg + "_out_len"] = lens.astype(np.float64)
+        arrays[leg + "_status"] = st.cpu().numpy().astype(np.float64)
+        arrays[leg + "_out_crc32"] = np.array([zlib.crc32(s) for s in streams], dtype=np.float64)
+        arrays[leg + "_sample_index"] = pick.astype(np.float64)
+        arrays[leg + "_sample_bytes"] = np.concatenate([streams[i] for i in pick]).astype(np.float32)
+        del host, streams
+    arrays["inflate_in_used"] = i_used.cpu().numpy().astype(np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, "--dump-outputs would write %d bytes" % total
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def main():
     out = _claim_stdout()
     ap = argparse.ArgumentParser()
@@ -266,7 +286,11 @@ def main():
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
     ap.add_argument("--small", action="store_true", help="1/8 size workload for quick checks (not a bench value)")
     ap.add_argument("--no-probe", dest="no_probe", action="store_true", help="(accepted for older command lines; no effect)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="write what the timed step computed in its last step to DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -395,6 +419,8 @@ def run_bench(args, rank, local_rank, world, out):
         sampler.start()
     ms_total = timed(step_resident, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dplan.out_offsets, d_dout, d_dlen, d_dst, iplan.out_offsets, d_iout, d_ilen, d_ist, d_iused)
     ms_step = ms_total / args.steps
     units_t = torch.tensor([float(U_def + U_inf)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -406,7 +432,7 @@ def run_bench(args, rank, local_rank, world, out):
     dplan.set_timing(True)
     iplan.set_timing(True)
     acc = {}
-    reps = max(3, min(args.steps, 5))
+    reps = args.steps
     for _ in range(reps):
         step_resident(overlap=False)  # one kernel at a time: these are per-kernel durations
         torch.cuda.synchronize()
@@ -420,7 +446,6 @@ def run_bench(args, rank, local_rank, world, out):
     peak, peak_src = peaks()
     alg_bytes = (C_inf + U_inf) if dom in INFLATE_KERNELS else (U_def + C_def)
     achieved = alg_bytes / (acc[dom] / 1e3) / 1e9
-    traffic, traffic_src = captured_traffic(dom, args.small)
     legs = {"deflate": {"ms": t_def, "algorithmic_bytes": U_def + C_def, "gbs": (U_def + C_def) / (t_def / 1e3) / 1e9 if t_def else None},
             "inflate": {"ms": t_inf, "algorithmic_bytes": C_inf + U_inf, "gbs": (C_inf + U_inf) / (t_inf / 1e3) / 1e9 if t_inf else None}}
     for v in legs.values():
@@ -492,7 +517,7 @@ def run_bench(args, rank, local_rank, world, out):
     hi = h_iout.numpy()
     for i in range(0, n_inf, max(1, n_inf // 8)):
         assert np.array_equal(hi[iout_off[i]:iout_off[i] + t_np[i].size], t_np[i]), "e2e inflate mismatch %d" % i
-    n_e2e = max(3, args.steps)
+    n_e2e = args.steps
     ms_e2e = timed_host(e2e_steps, n_e2e) / n_e2e
     e2e_val = units / (ms_e2e / 1e3) / 1e9
     # the same call on PAGEABLE host memory (what a caller that never pinned anything hands over): staged by the library
@@ -504,7 +529,7 @@ def run_bench(args, rank, local_rank, world, out):
     dout_p = P.pointers([pg_dout.ctypes.data + int(o) for o in dout_off])
     iout_p = P.pointers([pg_iout.ctypes.data + int(o) for o in iout_off])
     e2e_steps(2)
-    ms_pg = timed_host(e2e_steps, 3) / 3
+    ms_pg = timed_host(e2e_steps, args.steps) / args.steps
     dpipe.close()
     ipipe.close()
     del h_din, h_iin, h_dout, h_iout, pg_dout, pg_iout
@@ -566,7 +591,7 @@ def run_bench(args, rank, local_rank, world, out):
             "data": "synthetic",
             "config": {"workload": workload_name(N_DEFLATE // (8 if args.small else 1), N_INFLATE // (8 if args.small else 1)) if not strong
                        else "ONE C3 + C2 batch split over %d GPUs by bytes (rank 0: %d + %d buffers)" % (world, n_def, n_inf),
-                       "l2": "inputs (256 MiB + 77 MiB compressed per step) exceed the 126 MB L2; no flush needed",
+                       "l2": "inputs (256 MiB + 77 MiB compressed per step) exceed the 50 MB L2 of an H100; no flush needed",
                        "parity": "before timing: deflate bytes == oracle on 16 buffers, every inflated stream == original; e2e outputs checked again",
                        "ratio_deflate": U_def / max(1, C_def), "ratio_inflate": U_inf / max(1, C_inf), "setup_s": setup_s,
                        "inflate_pipeline": inflate_stats},
@@ -574,7 +599,7 @@ def run_bench(args, rank, local_rank, world, out):
             "inflate_gbs": U_inf / (t_inf / 1e3) / 1e9 if t_inf else None,
             "kernels_ms": acc, "legs": legs,
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "algorithmic_bytes": alg_bytes},
             "cpu_baseline": cpu,
             "e2e": {"value": e2e_val, "unit": "GB/s", "ms_per_step": ms_e2e,
@@ -597,7 +622,7 @@ def run_bench(args, rank, local_rank, world, out):
 
 
 def run_c4(args, rank, local_rank, world, out):
-    """BASELINE.json config 4: GZipOutputStream end to end (CRC32 + deflate) on ONE 2 GiB synthetic log stream, 1 x B200.
+    """BASELINE.json config 4: GZipOutputStream end to end (CRC32 + deflate) on ONE 2 GiB synthetic log stream, one GPU.
     The stream goes through the library's host call with wrap = GZIP (header, raw level-6 stream, CRC-32, ISIZE = 0x80000000);
     the bytes are compared with the oracle's for the whole stream (the reference's DeflaterEngine is serial: one host
     thread, ~80 s) and inflated back by zlib.  A single stream does not shard: other ranks idle ("replicas only")."""

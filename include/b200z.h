@@ -1,8 +1,8 @@
-/* b200z.h -- C-ABI of libb200z.so, the B200 (sm_100a) DEFLATE engine that replaces the managed inner loops of
+/* b200z.h -- C-ABI of libb200z.so, the H100 (sm_90a) DEFLATE engine that replaces the managed inner loops of
  * ICSharpCode.SharpZipLib.Zip.Compression.{Deflater,Inflater} and ICSharpCode.SharpZipLib.Checksum.{Crc32,Adler32}.
  *
  * Plain pointers and sizes only: this is what a P/Invoke (C#), ctypes (Python) or cgo binding declares.
- * Paths cited below are relative to /root/reference/src/ICSharpCode.SharpZipLib/ .
+ * Paths cited below are relative to SharpZipLib's src/ICSharpCode.SharpZipLib/ .
  *
  * Every function returns a b200z_status (0 = OK) unless noted; b200z_last_error() gives the message of the last
  * failure on the calling thread.  The status -> .NET exception mapping the C# shim applies is in INTEGRATION.md.

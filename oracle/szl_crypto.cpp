@@ -1,5 +1,5 @@
 // szl_crypto.cpp -- ORACLE (test infrastructure; never linked into the product): CPU restatement of the reference's
-// two entry ciphers, SURVEY.md row f4.  Paths are relative to /root/reference/src/ICSharpCode.SharpZipLib/.
+// two entry ciphers, SURVEY.md row f4.  Paths are relative to SharpZipLib's src/ICSharpCode.SharpZipLib/.
 //
 //   Encryption/ZipAESTransform.cs  :41-72  constructor: PBKDF2-HMAC-SHA1 (1000 rounds) -> key1 | key2 | 2-byte verifier
 //                                  :75-112 TransformBlock: AES-CTR, little-endian counter starting at 1, HMAC-SHA1 of the

@@ -2,7 +2,7 @@
 // Restates Checksum/{Adler32,Crc32,CrcUtilities}.cs and
 // Zip/Compression/{PendingBuffer,DeflaterPending,DeflaterConstants,DeflaterHuffman,
 // DeflaterEngine,Deflater}.cs of the reference (paths relative to
-// /root/reference/src/ICSharpCode.SharpZipLib/).  See szl_oracle.hpp for the pinning status.
+// SharpZipLib's src/ICSharpCode.SharpZipLib/).  See szl_oracle.hpp for the pinning status.
 #include "szl_oracle.hpp"
 #include <algorithm>
 #include <cstring>

@@ -1,7 +1,7 @@
 // szl_inflate.cpp -- ORACLE (test infrastructure): Inflater side.
 // Restates Zip/Compression/{Inflater,InflaterDynHeader,InflaterHuffmanTree}.cs and
 // Zip/Compression/Streams/{OutputWindow,StreamManipulator}.cs of the reference (paths relative
-// to /root/reference/src/ICSharpCode.SharpZipLib/).  See szl_oracle.hpp for the pinning status.
+// to SharpZipLib's src/ICSharpCode.SharpZipLib/).  See szl_oracle.hpp for the pinning status.
 #include "szl_oracle.hpp"
 #include <algorithm>
 #include <cstring>

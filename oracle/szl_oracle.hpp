@@ -8,7 +8,7 @@
 // This is a single-threaded C++17 restatement of the reference's managed C#
 // algorithm (ICSharpCode.SharpZipLib v1.4.2), following the reference's control
 // flow and variable names so it can be audited side by side.  Paths below are
-// relative to /root/reference/src/ICSharpCode.SharpZipLib/.
+// relative to SharpZipLib's src/ICSharpCode.SharpZipLib/.
 //
 // Pinning status (see DESIGN.md "Oracle"):
 //   * Crc32 / Adler32  : PINNED by the reference's known-answer tests

@@ -1,4 +1,4 @@
-"""sharpziplib_b200 -- host-side mirror of the SharpZipLib codec surface over libb200z.so (sm_100a kernels).
+"""sharpziplib_b200 -- host-side mirror of the SharpZipLib codec surface over libb200z.so (sm_90a kernels).
 
 Only the hot path is here: Deflater / Inflater / DeflaterOutputStream / InflaterInputStream / Crc32 / Adler32 and the
 batch plans the benchmark drives.  Names and argument meaning follow the reference (see each class's docstring for the

@@ -1,7 +1,7 @@
-// b200z_core.cuh -- per-thread building blocks of the B200 DEFLATE engine.
+// b200z_core.cuh -- per-thread building blocks of the H100 DEFLATE engine.
 //
 // Everything here is a __host__ __device__ inline function so that the same code that runs
-// inside the sm_100a kernels can be executed serially by tests/cpu_model (a g++-compiled harness
+// inside the sm_90a kernels can be executed serially by tests/cpu_model (a g++-compiled harness
 // that checks the *parallel decomposition* -- link table, per-position match table, parse state
 // machine, block planner, tree builder, bit emitter -- against the oracle without a GPU).
 //

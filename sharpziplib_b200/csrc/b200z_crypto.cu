@@ -1,5 +1,5 @@
 // b200z_crypto.cu -- SURVEY.md row f4: the two entry ciphers the reference applies to compressed bytes
-// (Streams/DeflaterOutputStream.cs:227-231 EncryptBlock; paths relative to /root/reference/src/ICSharpCode.SharpZipLib/).
+// (Streams/DeflaterOutputStream.cs:227-231 EncryptBlock; paths relative to SharpZipLib's src/ICSharpCode.SharpZipLib/).
 //
 //   WinZip AES   Encryption/ZipAESTransform.cs: constructor :41-72 (PBKDF2-HMAC-SHA1, 1000 rounds: key1 | key2 | verifier),
 //                TransformBlock :75-112 (AES-CTR, little-endian counter starting at 1; HMAC-SHA1 of the ciphertext),

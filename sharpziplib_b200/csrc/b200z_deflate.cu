@@ -1,4 +1,4 @@
-// b200z_deflate.cu -- the sm_100a DEFLATE compressor for the reference's lazy levels (5-9).
+// b200z_deflate.cu -- the sm_90a DEFLATE compressor for the reference's lazy levels (5-9).
 // Kernel decomposition and the reference lines each kernel replaces: see b200z_core.cuh and DESIGN.md.
 //
 //   k_links   (K1)  DeflaterEngine.InsertString / head[] / prev[]         DeflaterEngine.cs:417-439
@@ -201,9 +201,9 @@ __global__ void __launch_bounds__(kMatchThreads, 1)
 	// are bucketed by an estimate of their walk length (the first eight hops are exact, beyond that their hop density
 	// extrapolated over the window) and handed to the threads longest first: warps then hold walks of similar length.
 	// The order only decides who computes what; every position's result is unchanged.
-	// (Measured in round 2 and dropped: the walks as a flat state machine -- one candidate test or four bytes of extension per
-	// lane and iteration, free lanes refilled from the ordered list eight at a time.  Bit-exact, 41.5 ms instead of 21.2 ms on
-	// the bench workload: every iteration pays for every state's code.  profiles/README.md.)
+	// (Tried and dropped: the walks as a flat state machine -- one candidate test or four bytes of extension per lane and
+	// iteration, free lanes refilled from the ordered list eight at a time.  Bit-exact but slower on the bench workload:
+	// every iteration pays for every state's code.)
 	__shared__ uint32_t s_cls[2][kMatchClasses];
 	if (threadIdx.x < 2 * kMatchClasses) (&s_cls[0][0])[threadIdx.x] = 0;
 	__syncthreads();
@@ -369,7 +369,7 @@ __global__ void __launch_bounds__(kMatchThreads, 1)
 //            positions and records the block cuts (every 16384 symbols, DeflaterHuffman.cs:863).
 // ------------------------------------------------------------------------------------------------
 constexpr int kSegShift = 5;
-constexpr int kSeg = 1 << kSegShift; // 32 positions per lane: 9.6 KiB of shared memory per warp, 22 warps per SM (64: 4.5 ms, 32: 3.2 ms, 16: 3.4 ms)
+constexpr int kSeg = 1 << kSegShift; // 32 positions per lane: 9.6 KiB of shared memory per warp, 22 warps per SM
 constexpr int kRound = 32 * kSeg;
 constexpr int kParseWarm = 128; // positions a chunk parses in front of its first one to find its entry state (k_parse_chunk)
 constexpr int kSegStride = kSeg + 2; // uint2 entries; +2 keeps 16-byte alignment for cp.async and staggers the banks
@@ -1480,7 +1480,7 @@ int deflate_plan_build(b200z_plan *p) {
 	// length with the smallest estimate of waves x steps per run; B200Z_LINK_RUN=<positions> overrides it for timing.
 	p->link_run = kRun;
 	{
-		int sms = 148;
+		int sms = 132;
 		int dev = 0;
 		if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 		const int64_t slots = 3ll * sms;
@@ -1514,7 +1514,7 @@ int deflate_plan_build(b200z_plan *p) {
 		if (need <= 32768 && p->engine_state.empty()) pe = (int)((need + 255) / 256 * 256); // (a carried state holds whole tables)
 		p->fast_prev_entries = pe;
 		// persistent one-warp CTAs: as many per SM as their prev[] tables fit (head[] is in the pool), 16 at most
-		int sms = 148, dev = 0;
+		int sms = 132, dev = 0;
 		if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 		int per_sm = (int)((227 * 1024) / (2 * pe + 1024));
 		if (per_sm > 16) per_sm = 16;

@@ -1,4 +1,4 @@
-// b200z_inflate.cu -- the sm_100a DEFLATE decompressor.
+// b200z_inflate.cu -- the sm_90a DEFLATE decompressor.
 //
 // Replaces the reference's Inflater mode machine and its helpers:
 //   Inflater.Decode / DecodeHuffman          Zip/Compression/Inflater.cs:429-552, :283-386

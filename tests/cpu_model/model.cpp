@@ -1,5 +1,5 @@
 // model.cpp -- TEST INFRASTRUCTURE.  Serial host execution of the *kernel decomposition* in
-// sharpziplib_b200/csrc/b200z_core.cuh (the very same __host__ __device__ functions the sm_100a kernels call),
+// sharpziplib_b200/csrc/b200z_core.cuh (the very same __host__ __device__ functions the sm_90a kernels call),
 // so the exactness of the parallel reformulation can be checked against the oracle in the CPU-only test tier.
 // It is not a fallback: the product library never links it.
 #include "b200z_core.cuh"

@@ -17,7 +17,7 @@
 #include <functional>
 #include <vector>
 
-#define __CUDA_ARCH__ 1000
+#define __CUDA_ARCH__ 900
 #define B200Z_EMU 1
 #define __global__
 #define __device__

@@ -311,3 +311,26 @@ def test_bench_c4_c5_modes_run_small():
         else:
             assert d["all_parity"] and len(d["points"]) >= 18, d
     assert corpus_small()
+
+
+def test_bench_dump_outputs(tmp_path):
+    """bench.py --dump-outputs: the last timed step's outputs as float .npy files, within 64 MB, equal to what the oracle and
+    the generator say they are"""
+    import json
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--small", "--steps", "2", "--warmup", "1",
+                        "--dump-outputs", str(tmp_path)], capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, r.stderr[-3000:]
+    assert json.loads(r.stdout.strip().splitlines()[-1])["steps"] == 2
+    a = {f[:-4]: np.load(os.path.join(tmp_path, f)) for f in os.listdir(tmp_path)}
+    assert sum(os.path.getsize(os.path.join(tmp_path, f)) for f in os.listdir(tmp_path)) <= 64 << 20
+    assert all(v.dtype in (np.float32, np.float64) for v in a.values())
+    assert not a["deflate_status"].any() and not a["inflate_status"].any()
+    assert (a["inflate_out_len"] == 1 << 20).all()
+    i = int(a["inflate_sample_index"][0])
+    orig = datagen.text_buffer(i, 1 << 20, config=2).tobytes()
+    assert a["inflate_out_crc32"][i] == zlib.crc32(orig)
+    assert bytes(a["inflate_sample_bytes"][:1 << 20].astype(np.uint8)) == orig
+    j = int(a["deflate_sample_index"][0])
+    comp = bytes(a["deflate_sample_bytes"][:int(a["deflate_out_len"][j])].astype(np.uint8))
+    assert zlib.crc32(comp) == a["deflate_out_crc32"][j]
+    assert zlib.decompress(comp, -15) == datagen.silesia_mix(j, 262144, config=3).tobytes()

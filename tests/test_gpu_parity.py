@@ -1,4 +1,4 @@
-"""GPU tier (run with -m gpu on the B200 box): every CUDA path against the oracle, through the C-ABI."""
+"""GPU tier (run with -m gpu on an H100): every CUDA path against the oracle, through the C-ABI."""
 import io
 import json
 import os

@@ -1,4 +1,4 @@
-"""BASELINE.json configs 4 and 5 on one B200 (kernel-only device time through the plan API, bit-exactness spot-checked).
+"""BASELINE.json configs 4 and 5 on one GPU (kernel-only device time through the plan API, bit-exactness spot-checked).
 C4: GZipOutputStream semantics on one long log stream (raw deflate L6 + CRC32 on the device; the 18 header/trailer
     bytes are the host stream layer's).  C5: levels 1/6/9 x buffer sizes, 256 MiB per point (64 MiB x 4 at the top)."""
 import json

@@ -1,7 +1,7 @@
 // Golden-digest and timing harness for the REAL SharpZipLib (BASELINE.md section 2.1): runs the reference's own
 // Deflater / Inflater over buffer files written by tools/csharp_harness/export_inputs.py and prints, per buffer, the
-// SHA-256 of the compressed bytes, plus single-thread and N-thread throughput.  Needs a .NET SDK (>= 6.0); neither this
-// build container nor the GPU boxes of this pool have one (profiles/r02_probe_gpu_box.txt), so it ships as source:
+// SHA-256 of the compressed bytes, plus single-thread and N-thread throughput.  Needs a .NET SDK (>= 6.0), so it ships as
+// source:
 //   dotnet run -c Release --project tools/csharp_harness -- <dir with *.bin> <level> <threads> > reference_digests.json
 // tests/test_oracle.py::test_reference_digests compares oracle and GPU output with that file when it exists.
 using System;

@@ -1,4 +1,4 @@
-"""Small fixed workload for ncu captures of k_fast: NS x 256 KiB Silesia-mix at LEVEL (default 148 streams, level 1), two runs."""
+"""Small fixed workload for ncu captures of k_fast: NS x 256 KiB Silesia-mix at LEVEL (default 132 streams, one per H100 SM, level 1), two runs."""
 import os
 import sys
 
@@ -10,7 +10,7 @@ import sharpziplib_b200 as z  # noqa: E402
 from sharpziplib_b200 import datagen  # noqa: E402
 
 z.init(0)
-ns, level = int(os.environ.get("NS", "148")), int(os.environ.get("LEVEL", "1"))
+ns, level = int(os.environ.get("NS", "132")), int(os.environ.get("LEVEL", "1"))
 d_np = [datagen.silesia_mix(i % 32, 262144, config=5) for i in range(ns)]
 plan = z.DeflatePlan([a.size for a in d_np], level=level)
 h = np.zeros(plan.in_bytes, dtype=np.uint8)
