@@ -49,16 +49,23 @@ struct LevelParams {
 	int good, lazy, nice, chain, func;
 };
 
+constexpr int kLevelChain[10] = {0, 4, 8, 32, 16, 32, 128, 256, 1024, 4096}; // MAX_CHAIN, DeflaterConstants.cs:139
+// k_match tests the budgets of levels 5-9 (chain and chain >> 2) once per four candidates
+static_assert(kLevelChain[5] % 16 == 0 && kLevelChain[6] % 16 == 0 && kLevelChain[7] % 16 == 0 && kLevelChain[8] % 16 == 0 &&
+                  kLevelChain[9] % 16 == 0,
+              "level 5-9 chain budgets must be multiples of 16");
+
 B200Z_HD LevelParams level_params(int level) { // DeflaterConstants.cs:124-144
 	const int good[10] = {0, 4, 4, 4, 4, 8, 8, 8, 32, 32};
 	const int lazy[10] = {0, 4, 5, 6, 4, 16, 16, 32, 128, 258};
 	const int nice[10] = {0, 8, 16, 32, 16, 32, 128, 128, 258, 258};
-	const int chain[10] = {0, 4, 8, 32, 16, 32, 128, 256, 1024, 4096};
 	const int func[10] = {0, 1, 1, 1, 1, 2, 2, 2, 2, 2};
 	LevelParams lp;
 	lp.good = good[level];
 	lp.lazy = lazy[level];
 	lp.nice = nice[level];
+	const int chain[10] = {kLevelChain[0], kLevelChain[1], kLevelChain[2], kLevelChain[3], kLevelChain[4],
+	                       kLevelChain[5], kLevelChain[6], kLevelChain[7], kLevelChain[8], kLevelChain[9]}; // constant indices: usable on the device
 	lp.chain = chain[level];
 	lp.func = func[level];
 	return lp;

@@ -190,6 +190,19 @@ __global__ void __launch_bounds__(kMatchThreads, 1)
 	}
 	bulk_wait(&s_bar, 0);
 	__syncthreads();
+	// "No predecessor" (0) becomes a jump of 0xFFFF window positions: it lands below any position's lowest chain index
+	// (more than kMaxDist back), so one compare ends a walk at the chain's end and at the distance limit alike.
+	{
+		uint32_t *s_lw = reinterpret_cast<uint32_t *>(s_link);
+		const uint32_t nw = (t1 - w0 + 1) >> 1; // an odd count also rewrites the slot behind the last one: never staged, never read
+		for (uint32_t i = threadIdx.x; i < nw; i += kMatchThreads) {
+			uint32_t w = s_lw[i];
+			if ((w & 0xFFFFu) == 0) w |= 0xFFFFu;
+			if ((w >> 16) == 0) w |= 0xFFFF0000u;
+			s_lw[i] = w;
+		}
+	}
+	__syncthreads();
 	uint2 *out = mt + off;
 	// match_search() of b200z_core.cuh with the byte-wise extension loop replaced by 4-byte compares on aligned
 	// shared-memory words (ncu: the byte loop ran with ~2 of 32 lanes active and took ~30 % of the kernel).
@@ -224,7 +237,7 @@ __global__ void __launch_bounds__(kMatchThreads, 1)
 				uint32_t dist = d, hops = 1;
 				while (hops < 8) {
 					const uint32_t l2 = s_link[is - dist];
-					if (l2 == 0 || dist + l2 >= (uint32_t)kMaxDist) break;
+					if (dist + l2 >= (uint32_t)kMaxDist) break; // also the chain's end (0xFFFF)
 					dist += l2;
 					++hops;
 				}
@@ -269,86 +282,107 @@ __global__ void __launch_bounds__(kMatchThreads, 1)
 	__syncthreads();
 	for (uint32_t i = threadIdx.x; i < total; i += kMatchThreads) {
 		const uint32_t p = t0 + (uint32_t)__ldcg(&order[i]);
-		uint32_t resA = 0, resB = 0;
 		const uint32_t la = n - p;
-		const uint32_t d = (uint32_t)s_link[p - w0];
-		if (d != 0) {
-			const uint32_t maxlen = la < (uint32_t)kMaxMatch ? la : (uint32_t)kMaxMatch;
-			const uint32_t nice = la < (uint32_t)lp.nice ? la : (uint32_t)lp.nice;
-			const uint32_t is = p - w0;
-			const uint8_t *sp = s_data + is;
-			uint32_t m = kMinMatch - 1, bd = 0, dist = d, cnt = 0;
-			bool haveB = false;
-			uint32_t stop = budgetB ? budgetB : chain;
-			const uint32_t s0 = sp[0], s1 = sp[1];
-			uint32_t scan_end1 = s1, scan_end = sp[2];
-			// bytes 2..9 of the scan string stay in registers: most extensions end inside them
-			uint32_t sw0, sw1;
-			{
-				const uint32_t as = is + 2;
-				const uint32_t *ws = reinterpret_cast<const uint32_t *>(s_data + (as & ~3u));
-				const uint32_t w1 = ws[1], sh = (as & 3u) * 8u;
-				sw0 = __funnelshift_r(ws[0], w1, sh);
-				sw1 = __funnelshift_r(w1, ws[2], sh);
-			}
-			for (;;) {
-				const uint32_t ic = is - dist;
-				const uint8_t *c = s_data + ic;
-				++cnt;
-				if (c[m] == scan_end && c[m - 1] == scan_end1 && c[0] == s0 && c[1] == s1) {
-					uint32_t l = 2;
-					if (maxlen >= 10) {
-						const uint32_t ac = ic + 2;
-						const uint32_t *wc = reinterpret_cast<const uint32_t *>(s_data + (ac & ~3u));
-						const uint32_t w1 = wc[1], sh = (ac & 3u) * 8u;
-						uint32_t x = __funnelshift_r(wc[0], w1, sh) ^ sw0;
-						if (x) {
-							l = 2 + ((uint32_t)(__ffs((int)x) - 1) >> 3);
-							goto lcp_done;
-						}
-						x = __funnelshift_r(w1, wc[2], sh) ^ sw1;
-						if (x) {
-							l = 6 + ((uint32_t)(__ffs((int)x) - 1) >> 3);
-							goto lcp_done;
-						}
-						l = 10;
-					}
-					while (l + 4 <= maxlen) {
-						const uint32_t ac = ic + l, as = is + l;
-						const uint32_t *wc = reinterpret_cast<const uint32_t *>(s_data + (ac & ~3u));
-						const uint32_t *ws = reinterpret_cast<const uint32_t *>(s_data + (as & ~3u));
-						const uint32_t x = __funnelshift_r(wc[0], wc[1], (ac & 3u) * 8u) ^ __funnelshift_r(ws[0], ws[1], (as & 3u) * 8u);
-						if (x) {
-							l += (uint32_t)(__ffs((int)x) - 1) >> 3;
-							goto lcp_done;
-						}
-						l += 4;
-					}
-					while (l < maxlen && c[l] == sp[l]) ++l;
-				lcp_done:
-					if (l > m) {
-						m = l;
-						bd = dist;
-						if (m >= nice) break;
-						scan_end1 = sp[m - 1];
-						scan_end = sp[m];
-					}
-				}
-				if (cnt == stop) { // one test per candidate: first the quarter budget (B's snapshot), then the full one
-					if (stop == chain) break;
-					resB = m >= (uint32_t)kMinMatch ? pack_match(m, bd) : 0u;
-					haveB = true;
-					stop = chain;
-				}
-				const uint32_t l2 = s_link[is - dist];
-				if (l2 == 0) break;
-				dist += l2;
-				if (dist >= (uint32_t)kMaxDist) break; // chain entries need distance < 32506 (T7)
-			}
-			resA = m >= (uint32_t)kMinMatch ? pack_match(m, bd) : 0u;
-			if (!haveB) resB = resA;
+		const uint32_t maxlen = la < (uint32_t)kMaxMatch ? la : (uint32_t)kMaxMatch;
+		const uint32_t nice = la < (uint32_t)lp.nice ? la : (uint32_t)lp.nice;
+		const int is = (int)(p - w0);
+		const uint8_t *sp = s_data + is;
+		// The walk runs on window indices, offset by m so that the hot loop addresses the candidate's byte m directly:
+		// icm = candidate + m, lom = lo + m with lo the lowest index a later chain member may have (distance < 32506, T7),
+		// lk = the link window shifted by -m.  The re-encoded chain end lands below lo as well, so one compare per hop
+		// ends the walk.  A listed position always has a first candidate (see above).
+		uint32_t m = kMinMatch - 1, bd = 0, resB = 0;
+		int icm = is - (int)s_link[is] + (int)m;
+		int lom = is - (kMaxDist - 1) + (int)m;
+		const uint16_t *lk = s_link - m;
+		bool haveB = false;
+		uint32_t stop = budgetB ? budgetB : chain;
+		uint32_t left = stop; // candidates to test before the next budget event
+		const uint32_t s0 = sp[0], s1 = sp[1];
+		uint32_t scan_end1 = s1, scan_end = sp[2];
+		// bytes 2..9 of the scan string stay in registers: most extensions end inside them
+		uint32_t sw0, sw1;
+		{
+			const uint32_t as = (uint32_t)is + 2;
+			const uint32_t *ws = reinterpret_cast<const uint32_t *>(s_data + (as & ~3u));
+			const uint32_t w1 = ws[1], sh = (as & 3u) * 8u;
+			sw0 = __funnelshift_r(ws[0], w1, sh);
+			sw1 = __funnelshift_r(w1, ws[2], sh);
 		}
-		out[p] = make_uint2(resA, resB);
+		// Every level 5-9 budget (chain and chain >> 2) is a multiple of four: the walk steps four candidates per budget
+		// test (b200z_core.cuh asserts it).  The lanes of a warp step their candidates together; only a candidate whose
+		// byte m matches leaves the straight path.  (Tried and dropped: the rejects in a loop of their own, without the
+		// convergence region around the rare path -- fewer instructions, but the lanes no longer step together: DESIGN.md §7b.)
+		for (;;) {
+#pragma unroll
+			for (int j = 0; j < 4; j++) {
+				const uint32_t b = s_data[icm];
+				int nx = icm - (int)lk[icm];
+				if (b == scan_end) {
+					const int ic = icm - (int)m;
+					const uint8_t *c = s_data + ic;
+					// the other three bytes of the quick test in one branch: their loads are issued together
+					if ((c[m - 1] == scan_end1) & (c[0] == s0) & (c[1] == s1)) {
+						uint32_t l = 2;
+						if (maxlen >= 10) {
+							const uint32_t ac = (uint32_t)ic + 2;
+							const uint32_t *wc = reinterpret_cast<const uint32_t *>(s_data + (ac & ~3u));
+							const uint32_t w1 = wc[1], sh = (ac & 3u) * 8u;
+							uint32_t x = __funnelshift_r(wc[0], w1, sh) ^ sw0;
+							if (x) {
+								l = 2 + ((uint32_t)(__ffs((int)x) - 1) >> 3);
+								goto lcp_done;
+							}
+							x = __funnelshift_r(w1, wc[2], sh) ^ sw1;
+							if (x) {
+								l = 6 + ((uint32_t)(__ffs((int)x) - 1) >> 3);
+								goto lcp_done;
+							}
+							l = 10;
+						}
+						while (l + 4 <= maxlen) {
+							const uint32_t ac = (uint32_t)ic + l, as = (uint32_t)is + l;
+							const uint32_t *wc = reinterpret_cast<const uint32_t *>(s_data + (ac & ~3u));
+							const uint32_t *ws = reinterpret_cast<const uint32_t *>(s_data + (as & ~3u));
+							const uint32_t x = __funnelshift_r(wc[0], wc[1], (ac & 3u) * 8u) ^ __funnelshift_r(ws[0], ws[1], (as & 3u) * 8u);
+							if (x) {
+								l += (uint32_t)(__ffs((int)x) - 1) >> 3;
+								goto lcp_done;
+							}
+							l += 4;
+						}
+						while (l < maxlen && c[l] == sp[l]) ++l;
+					lcp_done:
+						if (l > m) {
+							bd = (uint32_t)(is - ic);
+							if (l >= nice) {
+								m = l;
+								goto done;
+							}
+							nx += (int)(l - m);
+							lom += (int)(l - m);
+							lk -= l - m;
+							m = l;
+							scan_end1 = sp[m - 1];
+							scan_end = sp[m];
+						}
+					}
+				}
+				icm = nx;
+				if (icm < lom) goto done;
+			}
+			left -= 4;
+			if (left == 0) { // first the quarter budget (B's snapshot), then the full one
+				if (stop == chain) break;
+				resB = m >= (uint32_t)kMinMatch ? pack_match(m, bd) : 0u;
+				haveB = true;
+				left = chain - stop;
+				stop = chain;
+			}
+		}
+	done:
+		const uint32_t resA = m >= (uint32_t)kMinMatch ? pack_match(m, bd) : 0u;
+		out[p] = make_uint2(resA, haveB ? resB : resA);
 	}
 }
 
