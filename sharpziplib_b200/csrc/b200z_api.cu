@@ -63,11 +63,10 @@ int Arena::alloc() {
 		set_error("cudaMalloc of %lld workspace bytes failed: %s", (long long)size, cudaGetErrorString(e));
 		return B200Z_E_NOMEM;
 	}
+	for (const auto &u : pending)
+		if (!u.second.empty()) B200Z_CUDA(cudaMemcpy(base + u.first, u.second.data(), u.second.size(), cudaMemcpyHostToDevice));
+	pending.clear();
 	return B200Z_OK;
-}
-void Arena::release() {
-	if (base) cudaFree(base);
-	base = nullptr;
 }
 
 // ---- static tables blob ---------------------------------------------------------------------------
@@ -336,99 +335,7 @@ int b200z_deflate_plan_create_ex(int32_t n, const int64_t *in_len, int level, in
 	int rc = ensure_init();
 	if (rc) return rc;
 	DeviceGuard guard(current_device());
-	b200z_plan *p = new b200z_plan();
-	p->device = current_device();
-	p->kind = 0;
-	p->n = n;
-	p->level = level;
-	p->strategy = strategy;
-	p->wrap = wrap;
-	p->end_mode = end_mode;
-	p->in_len.assign(in_len, in_len + n);
-	if (hist && n > 0 && level <= 4) {
-		// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
-		if (hist->chunk_count) {
-			if (!hist->chunk_len) {
-				set_error("history: chunk_count without chunk_len");
-				delete p;
-				return B200Z_E_ARG;
-			}
-			p->sched_cum.resize(n);
-			for (int i = 0; i < n; i++) {
-				int64_t sum = 0;
-				for (int k = 0; k < hist->chunk_count[i]; k++) {
-					const int64_t c = hist->chunk_len[i] ? hist->chunk_len[i][k] : -1;
-					if (c < 0) {
-						set_error("stream %d: SetInput size %d", i, k);
-						delete p;
-						return B200Z_E_ARG;
-					}
-					sum += c;
-					p->sched_cum[i].push_back((uint32_t)sum);
-				}
-				if (hist->chunk_count[i] < 0 || (hist->chunk_count[i] > 0 && sum != in_len[i])) {
-					set_error("stream %d: the SetInput sizes add up to %lld, the stream has %lld bytes", i, (long long)sum,
-					          (long long)in_len[i]);
-					delete p;
-					return B200Z_E_ARG;
-				}
-			}
-		}
-		if (hist->undrained_last) p->undrained.assign(hist->undrained_last, hist->undrained_last + n);
-		if (hist->engine_state && level >= 1) p->engine_state.assign(hist->engine_state, hist->engine_state + n);
-		if (hist->stored_state && level == 0) p->stored_state = hist->stored_state;
-	}
-	if (hist && hist->kind != B200Z_HIST_NONE && n > 0) {
-		if ((hist->kind != B200Z_HIST_DICTIONARY && hist->kind != B200Z_HIST_CONTINUE) || !hist->hist_len) {
-			set_error("history: kind/hist_len");
-			delete p;
-			return B200Z_E_ARG;
-		}
-		if (hist->kind == B200Z_HIST_CONTINUE && level < 5) {
-			// DeflateStored / DeflateFast keep window-relative state across Deflate() calls that is not a function of the
-			// stream position: it has to come from the run of the previous segment
-			bool have = level == 0 ? p->stored_state != nullptr : !p->engine_state.empty();
-			for (void *q : p->engine_state) have = have && q != nullptr;
-			if (!have) {
-				set_error("continuing a stream after Flush() at levels 0-4 needs the engine state of the previous segment "
-				          "(b200z_history.engine_state / stored_state)");
-				delete p;
-				return B200Z_E_UNSUPPORTED;
-			}
-		}
-		p->hist_kind = hist->kind;
-		p->check_seeded = hist->check_seeded != 0;
-		p->hist.assign(hist->hist_len, hist->hist_len + n);
-		p->pos_base.resize(n);
-		p->bit_base.resize(n);
-		p->hist_mask.resize(n);
-		for (int i = 0; i < n; i++) {
-			const int64_t H = p->hist[i];
-			if (H < 0 || H > 32768 || (hist->kind == B200Z_HIST_DICTIONARY && H > kMaxDist)) {
-				set_error("stream %d: history of %lld bytes (at most %d)", i, (long long)H,
-				          hist->kind == B200Z_HIST_DICTIONARY ? kMaxDist : 32768);
-				delete p;
-				return B200Z_E_ARG;
-			}
-			p->pos_base[i] = (hist->pos_base && hist->kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
-			p->bit_base[i] = hist->bit_base ? hist->bit_base[i] : 0;
-			if (p->pos_base[i] < H || p->pos_base[i] > 0xFFFF0000ll || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
-				set_error("stream %d: pos_base/bit_base", i);
-				delete p;
-				return B200Z_E_ARG;
-			}
-			if (hist->hist_mask && hist->hist_mask[i]) p->hist_mask[i].assign(hist->hist_mask[i], hist->hist_mask[i] + H);
-			p->in_len[i] += H; // the input slot holds history + data
-		}
-	}
-	rc = deflate_plan_build(p);
-	if (rc) {
-		p->ws.release();
-		delete p;
-		return rc;
-	}
-	*plan = p;
-	return B200Z_OK;
+	return deflate_plan_create(n, in_len, level, strategy, wrap, end_mode, hist, plan);
 }
 
 int b200z_inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, b200z_plan **plan) {
@@ -444,33 +351,7 @@ int b200z_inflate_plan_create_ex(int32_t n, const int64_t *comp_len, const int64
 	int rc = ensure_init();
 	if (rc) return rc;
 	DeviceGuard guard(current_device());
-	b200z_plan *p = new b200z_plan();
-	p->device = current_device();
-	p->kind = 1;
-	p->n = n;
-	p->wrap = wrap;
-	p->in_len.assign(comp_len, comp_len + n);
-	p->out_cap.assign(out_cap, out_cap + n);
-	if (dict_len && n > 0) {
-		p->hist_kind = B200Z_HIST_DICTIONARY;
-		p->hist.assign(dict_len, dict_len + n);
-		for (int i = 0; i < n; i++) {
-			if (p->hist[i] < 0 || p->hist[i] > 32768) { // OutputWindow.CopyDict keeps the last WindowSize bytes (:160-166)
-				set_error("stream %d: dictionary of %lld bytes (at most 32768)", i, (long long)p->hist[i]);
-				delete p;
-				return B200Z_E_ARG;
-			}
-			p->in_len[i] += p->hist[i];
-		}
-	}
-	rc = inflate_plan_build(p);
-	if (rc) {
-		p->ws.release();
-		delete p;
-		return rc;
-	}
-	*plan = p;
-	return B200Z_OK;
+	return inflate_plan_create(n, comp_len, out_cap, wrap, dict_len, plan);
 }
 
 int b200z_inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit) {
@@ -483,17 +364,13 @@ int b200z_inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit
 		set_error("start bits are for raw streams (a framed stream starts behind its header)");
 		return B200Z_E_ARG;
 	}
-	std::vector<uint32_t> sb((size_t)plan->n);
 	for (int i = 0; i < plan->n; i++) {
 		if (start_bit[i] < 0 || start_bit[i] > 7) {
 			set_error("stream %d: start bit %d (0..7)", i, start_bit[i]);
 			return B200Z_E_ARG;
 		}
-		sb[(size_t)i] = (uint32_t)start_bit[i];
 	}
-	if (plan->n) B200Z_CUDA(cudaMemcpy(plan->ws.at<uint32_t>(plan->o_start_bit), sb.data(), 4ull * plan->n, cudaMemcpyHostToDevice));
-	plan->has_start_bits = true;
-	return B200Z_OK;
+	return inflate_plan_set_start_bits(plan, start_bit);
 }
 
 int b200z_inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, const int64_t *dict_len) {
@@ -502,29 +379,7 @@ int b200z_inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, co
 		set_error("bad arguments");
 		return B200Z_E_ARG;
 	}
-	const int n = plan->n;
-	std::vector<int64_t> dl((size_t)n);
-	std::vector<uint32_t> d32((size_t)n);
-	for (int i = 0; i < n; i++) {
-		const int64_t D = dict_len ? dict_len[i] : 0;
-		if (comp_len[i] < 0 || comp_len[i] > plan->comp_cap[(size_t)i] || D < 0 || D > plan->dict_cap[(size_t)i]) {
-			set_error("stream %d: %lld compressed / %lld dictionary bytes exceed what the plan was created for (%lld / %lld)", i,
-			          (long long)comp_len[i], (long long)D, (long long)plan->comp_cap[(size_t)i], (long long)plan->dict_cap[(size_t)i]);
-			return B200Z_E_ARG;
-		}
-		dl[(size_t)i] = comp_len[i];
-		d32[(size_t)i] = (uint32_t)D;
-	}
-	for (int i = 0; i < n; i++) { // the dictionary ends where the compressed bytes start
-		if (!plan->hist.empty()) plan->hist[(size_t)i] = d32[(size_t)i];
-		plan->in_off[(size_t)i] = plan->comp_off[(size_t)i] - d32[(size_t)i];
-		plan->in_len[(size_t)i] = comp_len[i] + d32[(size_t)i];
-	}
-	if (n) {
-		B200Z_CUDA(cudaMemcpy(plan->ws.at<int64_t>(plan->o_in_len), dl.data(), 8ull * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(plan->ws.at<uint32_t>(plan->o_hist), d32.data(), 4ull * n, cudaMemcpyHostToDevice));
-	}
-	return B200Z_OK;
+	return inflate_plan_set_lengths(plan, comp_len, dict_len);
 }
 
 int b200z_plan_get_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_pos, void *cuda_stream) {
@@ -534,15 +389,7 @@ int b200z_plan_get_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_p
 		return B200Z_E_ARG;
 	}
 	if (plan->n == 0) return B200Z_OK;
-	std::vector<int64_t> rp(2 * (size_t)plan->n);
-	cudaStream_t s = (cudaStream_t)cuda_stream;
-	B200Z_CUDA(cudaMemcpyAsync(rp.data(), plan->ws.at<int64_t>(plan->o_restart), 16ull * plan->n, cudaMemcpyDeviceToHost, s));
-	B200Z_CUDA(cudaStreamSynchronize(s));
-	for (int i = 0; i < plan->n; i++) {
-		bit[i] = rp[2 * (size_t)i];
-		out_pos[i] = rp[2 * (size_t)i + 1];
-	}
-	return B200Z_OK;
+	return inflate_plan_restart_points(plan, bit, out_pos, (cudaStream_t)cuda_stream);
 }
 
 int b200z_plan_get_stats(b200z_plan *plan, uint32_t *v, int32_t cap, void *cuda_stream) {
@@ -584,9 +431,6 @@ int b200z_plan_get_timings(b200z_plan *plan, char *names, int32_t names_cap, flo
 
 int b200z_plan_destroy(b200z_plan *plan) {
 	DeviceGuard guard(plan ? plan->device : -1);
-	if (!plan) return B200Z_OK;
-	for (cudaEvent_t e : plan->ev) cudaEventDestroy(e);
-	plan->ws.release();
 	delete plan;
 	return B200Z_OK;
 }
@@ -675,7 +519,7 @@ extern "C" int b200z_plan_pack(b200z_plan *plan, const uint8_t *d_out, const int
 	if (plan->n == 0) return B200Z_OK;
 	cudaStream_t s = (cudaStream_t)cuda_stream;
 	k_pack_offsets<<<1, 1024, 0, s>>>(plan->n, d_out_len, d_packed_off);
-	k_pack<<<plan->n, 256, 0, s>>>(d_out, plan->ws.at<int64_t>(plan->o_out_off), d_out_len, d_packed_off, d_packed);
+	k_pack<<<plan->n, 256, 0, s>>>(d_out, plan->dev_out_off(), d_out_len, d_packed_off, d_packed);
 	B200Z_CUDA(cudaGetLastError());
 	return B200Z_OK;
 }
@@ -1384,9 +1228,9 @@ static int deflater_run_device(DeflaterH *d, int end_mode) {
 		inp = slot.data();
 	}
 	HostRunResult r;
-	const uint32_t seed = d->adler;
+	const uint32_t seed = d->adler; // a plan with history continues the running checksum (hs.check_seeded)
 	rc = run_plan_host(plan, &inp, d->hin, d->hout, d->din, d->dout, d->dmeta, r, false,
-	                   (plan->check_seeded && !d->raw) ? &seed : nullptr);
+	                   (hs.kind != B200Z_HIST_NONE && !d->raw) ? &seed : nullptr);
 	if (!rc && (r.status[0] & 0xFF) != B200Z_OK) {
 		rc = r.status[0] & 0xFF;
 		set_error("device deflate failed with status %d", rc);

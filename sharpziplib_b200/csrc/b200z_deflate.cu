@@ -9,6 +9,8 @@
 //   k_emit    (K6)  SendAllTrees / CompressBlock / FlushStoredBlock       DeflaterHuffman.cs:676-779
 #include <cuda_pipeline.h>
 
+#include <memory>
+
 #include "b200z_internal.cuh"
 #include "b200z_tma.cuh"
 
@@ -1486,7 +1488,49 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-int deflate_plan_build(b200z_plan *p) {
+struct DeflatePlan final : b200z_plan {
+	// with history (b200z_deflate_plan_create_ex)
+	int hist_kind = 0; // B200Z_HIST_*
+	bool check_seeded = false;
+	std::vector<int64_t> pos_base;
+	std::vector<int32_t> bit_base;
+	std::vector<std::vector<uint8_t>> hist_mask;
+	// levels 0-4: the SetInput schedule of every stream (cumulative sizes), "Flush()/Finish() behind an undrained SetInput",
+	// and the engine state carried between the segments of a stream (b200z_history)
+	std::vector<std::vector<uint32_t>> sched_cum;
+	std::vector<int32_t> undrained;
+	std::vector<void *> engine_state;           // device pointers (levels 1-4)
+	b200z_stored_state *stored_state = nullptr; // caller's host array (level 0), used while the plan is built
+	int n_runs = 0, n_tiles = 0, n_blkmax = 0, n_chunks = 0, n_rgroups = 0, n_stored = 0, n_ck_tiles = 0;
+	uint32_t parse_chunk = 32768;
+	int link_run = 65536; // positions per k_links CTA (B200Z_LINK_RUN)
+	int fast_prev_entries = 32768; // k_fast's prev[] size for this batch
+	int fast_ctas = 1;             // k_fast's persistent CTAs (each owns a head[] slot of the pool)
+	bool fast_head_smem = false;   // ... or keeps head[] in shared memory (few streams)
+	// workspace (deflate_plan_build lays it out)
+	Slot<uint32_t> o_blk_off, o_nsyms, o_nblocks, o_blk_start, o_blk_ptop, o_sym, o_hist, o_bitbase;
+	Slot<int64_t> o_bias, o_hm_off, o_ck_off, o_ck_len;
+	Slot<int2> o_run_desc, o_tile_desc, o_rgroups;
+	Slot<int32_t> o_blk_desc;
+	Slot<BlockMeta> o_meta;
+	Slot<BlockTables> o_tables;
+	Slot<uint8_t> o_hmask;
+	Slot<CkTile> o_ck_desc;
+	Slot<unsigned long long> o_ck_acc;
+	Slot<uint16_t> o_link; // levels 5-9
+	Slot<uint2> o_mt;
+	Slot<uint32_t> o_sym_local, o_rnd_off, o_rnd_symoff;
+	Slot<ChunkDesc> o_chunks;
+	Slot<RoundRec> o_recs, o_ents;
+	Slot<StoredBlock> o_stored; // level 0
+	Slot<int64_t> o_slens;
+	Slot<uint32_t> o_sched, o_sched_off, o_fcounter; // levels 1-4
+	Slot<int32_t> o_undrained;
+	Slot<uint8_t *> o_fstate;
+	Slot<uint16_t> o_fhead;
+};
+
+static int deflate_plan_build(DeflatePlan *p) {
 	const LevelParams lp = level_params(p->level);
 	const int n = p->n;
 	std::vector<StoredBlock> sblocks; // level 0 only
@@ -1501,6 +1545,8 @@ int deflate_plan_build(b200z_plan *p) {
 	uint32_t nrounds = 0;
 	int64_t maxlen = 0;
 	for (int i = 0; i < n; i++) maxlen = p->in_len[i] > maxlen ? p->in_len[i] : maxlen;
+	int sms = 0;
+	if (sm_count(&sms) != cudaSuccess) sms = 132;
 	// chunk of the parse: 32 Ki positions (one warp each); k_parse_fix only compares states at their boundaries, so a long
 	// stream may have tens of thousands of them (grown beyond 65536 chunks per stream)
 	uint32_t chunk = 32768;
@@ -1514,9 +1560,6 @@ int deflate_plan_build(b200z_plan *p) {
 	// length with the smallest estimate of waves x steps per run; B200Z_LINK_RUN=<positions> overrides it for timing.
 	p->link_run = kRun;
 	{
-		int sms = 132;
-		int dev = 0;
-		if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 		const int64_t slots = 3ll * sms;
 		double best = 0;
 		for (int64_t run = 65536; run <= 1048576; run *= 2) {
@@ -1548,8 +1591,6 @@ int deflate_plan_build(b200z_plan *p) {
 		if (need <= 32768 && p->engine_state.empty()) pe = (int)((need + 255) / 256 * 256); // (a carried state holds whole tables)
 		p->fast_prev_entries = pe;
 		// persistent one-warp CTAs: as many per SM as their prev[] tables fit (head[] is in the pool), 16 at most
-		int sms = 132, dev = 0;
-		if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 		int per_sm = (int)((227 * 1024) / (2 * pe + 1024));
 		if (per_sm > 16) per_sm = 16;
 		if (per_sm < 1) per_sm = 1;
@@ -1563,7 +1604,7 @@ int deflate_plan_build(b200z_plan *p) {
 	uint32_t nblk = 0;
 	const bool has_hist = !p->hist.empty();
 	std::vector<uint32_t> hist32(n, 0u), bitbase32(n, 0u);
-	std::vector<int64_t> bias64(n, 0), hm_off(n, 0), ck_off(n), ck_len(n);
+	std::vector<int64_t> bias64(n, 0), hm_off(n, 0);
 	std::vector<uint8_t> hmask;
 	std::vector<int64_t> stored_taken(n, -1);
 	for (int i = 0; i < n; i++) {
@@ -1646,115 +1687,74 @@ int deflate_plan_build(b200z_plan *p) {
 	p->n_tiles = (int)tiles.size();
 	p->n_blkmax = (int)nblk;
 	Arena &ws = p->ws;
-	p->o_in_off = ws.reserve(8ll * n);
-	p->o_in_len = ws.reserve(8ll * n);
-	p->o_out_off = ws.reserve(8ll * n);
-	p->o_out_cap = ws.reserve(8ll * n);
-	p->o_run_desc = ws.reserve(8ll * (runs.size() + 1));
-	p->o_tile_desc = ws.reserve(8ll * (tiles.size() + 1));
-	p->o_blk_desc = ws.reserve(4ll * (nblk + 1));
-	p->o_blk_off = ws.reserve(4ll * (n + 1));
-	p->o_nsyms = ws.reserve(4ll * n);
-	p->o_nblocks = ws.reserve(4ll * n);
-	p->o_blk_start = ws.reserve(4ll * (nblk + 1));
-	p->o_blk_ptop = ws.reserve(4ll * (nblk + 1));
-	p->o_meta = ws.reserve((int64_t)sizeof(BlockMeta) * (nblk + 1));
-	p->o_tables = ws.reserve((int64_t)sizeof(BlockTables) * (nblk + 1));
+	p->upload_streams(p->in_off, p->in_len, 0);
+	p->o_run_desc = ws.upload(runs, 1);
+	p->o_tile_desc = ws.upload(tiles, 1);
+	p->o_blk_desc = ws.upload(blk_desc, 1);
+	p->o_blk_off = ws.upload(blk_off);
+	p->o_nsyms = ws.reserve<uint32_t>(n);
+	p->o_nblocks = ws.reserve<uint32_t>(n);
+	p->o_blk_start = ws.reserve<uint32_t>(nblk + 1);
+	p->o_blk_ptop = ws.reserve<uint32_t>(nblk + 1);
+	p->o_meta = ws.reserve<BlockMeta>(nblk + 1);
+	p->o_tables = ws.reserve<BlockTables>(nblk + 1);
 	if (lp.func == 2) {
-		p->o_link = ws.reserve(2ll * io + 64);
-		p->o_mt = ws.reserve(8ll * io + 64);
-		p->o_sym_local = ws.reserve(4ll * io + 64);
-		p->o_chunks = ws.reserve((int64_t)sizeof(ChunkDesc) * (chunks.size() + 1));
-		p->o_rgroups = ws.reserve(8ll * (rgroups.size() + 1));
-		p->o_rnd_off = ws.reserve(4ll * (n + 1));
-		p->o_recs = ws.reserve((int64_t)sizeof(RoundRec) * (nrounds + 1));
-		p->o_ents = ws.reserve((int64_t)sizeof(RoundRec) * (nrounds + 1));
-		p->o_rnd_symoff = ws.reserve(4ll * (nrounds + 1));
+		p->o_link = ws.reserve<uint16_t>(io + 32);
+		p->o_mt = ws.reserve<uint2>(io + 8);
+		p->o_sym_local = ws.reserve<uint32_t>(io + 16);
+		p->o_chunks = ws.upload(chunks, 1);
+		p->o_rgroups = ws.upload(rgroups, 1);
+		p->o_rnd_off = ws.upload(rnd_off);
+		p->o_recs = ws.reserve<RoundRec>(nrounds + 1);
+		p->o_ents = ws.reserve<RoundRec>(nrounds + 1);
+		p->o_rnd_symoff = ws.reserve<uint32_t>(nrounds + 1);
 	}
-	if (lp.func != 0) p->o_sym = ws.reserve(4ll * io + 64);
+	if (lp.func != 0) p->o_sym = ws.reserve<uint32_t>(io + 16);
 	if (lp.func == 0) {
 		p->n_stored = (int)sblocks.size();
-		p->o_stored = ws.reserve((int64_t)sizeof(StoredBlock) * (sblocks.size() + 1));
-		p->o_slens = ws.reserve(8ll * (n + 1));
+		p->o_stored = ws.upload(sblocks, 1);
+		p->o_slens = ws.upload(slens, 1);
 	}
-	std::vector<uint32_t> sched_flat, sched_off(n + 1, 0u);
-	std::vector<int32_t> undrained32(n, 0);
-	std::vector<void *> fstate(n, nullptr);
 	if (lp.func == 1) {
+		std::vector<uint32_t> sched_flat, sched_off(n + 1, 0u);
+		std::vector<int32_t> undrained32(n, 0);
+		std::vector<uint8_t *> fstate(n, nullptr);
 		for (int i = 0; i < n; i++) {
 			sched_off[i] = (uint32_t)sched_flat.size();
 			if (i < (int)p->sched_cum.size()) sched_flat.insert(sched_flat.end(), p->sched_cum[i].begin(), p->sched_cum[i].end());
 			if (i < (int)p->undrained.size()) undrained32[i] = p->undrained[i] ? 1 : 0;
-			if (i < (int)p->engine_state.size()) fstate[i] = p->engine_state[i];
+			if (i < (int)p->engine_state.size()) fstate[i] = static_cast<uint8_t *>(p->engine_state[i]);
 		}
 		sched_off[n] = (uint32_t)sched_flat.size();
-		p->o_sched = ws.reserve(4ll * (sched_flat.size() + 1));
-		p->o_sched_off = ws.reserve(4ll * (n + 1));
-		p->o_undrained = ws.reserve(4ll * (n + 1));
-		p->o_fstate = ws.reserve(8ll * (n + 1));
-		p->o_fhead = ws.reserve(p->fast_head_smem ? 256 : 65536ll * p->fast_ctas);
-		p->o_fcounter = ws.reserve(256);
+		p->o_sched = ws.upload(sched_flat, 1);
+		p->o_sched_off = ws.upload(sched_off);
+		p->o_undrained = ws.upload(undrained32, 1);
+		p->o_fstate = ws.upload(fstate, 1);
+		p->o_fhead = ws.reserve<uint16_t>(p->fast_head_smem ? 128 : 32768ll * p->fast_ctas);
+		p->o_fcounter = ws.reserve<uint32_t>(64);
 	}
-	p->o_hist = ws.reserve(4ll * (n + 1));
-	p->o_bias = ws.reserve(8ll * (n + 1));
-	p->o_bitbase = ws.reserve(4ll * (n + 1));
-	p->o_hm_off = ws.reserve(8ll * (n + 1));
-	p->o_hmask = ws.reserve((int64_t)hmask.size() + 16);
-	std::vector<CkTile> ck_tiles;
+	p->o_hist = ws.upload(hist32, 1);
+	p->o_bias = ws.upload(bias64, 1);
+	p->o_bitbase = ws.upload(bitbase32, 1);
+	p->o_hm_off = ws.upload(hm_off, 1);
+	p->o_hmask = ws.upload(hmask, 16);
 	if (p->wrap != B200Z_WRAP_RAW) {
+		std::vector<int64_t> ck_off(n), ck_len(n);
 		for (int i = 0; i < n; i++) { // the checksum covers the data, never the history
 			ck_off[i] = p->in_off[i] + hist32[i];
 			ck_len[i] = p->in_len[i] - hist32[i];
 			if (stored_taken[i] >= 0 && stored_taken[i] < ck_len[i]) ck_len[i] = stored_taken[i]; // level 0, see above
 		}
-		p->o_ck_off = ws.reserve(8ll * (n + 1));
-		p->o_ck_len = ws.reserve(8ll * (n + 1));
+		p->o_ck_off = ws.upload(ck_off, 1);
+		p->o_ck_len = ws.upload(ck_len, 1);
+		std::vector<CkTile> ck_tiles;
 		checksum_tiles(ck_len.data(), n, ck_tiles, p->wrap == B200Z_WRAP_ZLIB ? 1 : 0);
 		p->n_ck_tiles = (int)ck_tiles.size();
-		p->o_ck_desc = ws.reserve((int64_t)sizeof(CkTile) * (ck_tiles.size() + 1));
-		p->o_ck_acc = ws.reserve(16ll * (n + 1));
+		p->o_ck_desc = ws.upload(ck_tiles, 1);
+		p->o_ck_acc = ws.reserve<unsigned long long>(2ll * (n + 1));
 	}
 	int rc = ws.alloc();
 	if (rc) return rc;
-	B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_in_off), p->in_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-	B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_in_len), p->in_len.data(), 8ll * n, cudaMemcpyHostToDevice));
-	B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_out_off), p->out_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-	B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_out_cap), p->out_cap.data(), 8ll * n, cudaMemcpyHostToDevice));
-	if (n) {
-		B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_hist), hist32.data(), 4ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_bias), bias64.data(), 8ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_bitbase), bitbase32.data(), 4ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_hm_off), hm_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-		if (!hmask.empty()) B200Z_CUDA(cudaMemcpy(ws.at<uint8_t>(p->o_hmask), hmask.data(), hmask.size(), cudaMemcpyHostToDevice));
-		if (p->wrap != B200Z_WRAP_RAW) {
-			B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_ck_off), ck_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-			B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_ck_len), ck_len.data(), 8ll * n, cudaMemcpyHostToDevice));
-		}
-	}
-	if (!runs.empty()) B200Z_CUDA(cudaMemcpy(ws.at<int2>(p->o_run_desc), runs.data(), 8ll * runs.size(), cudaMemcpyHostToDevice));
-	if (!tiles.empty()) B200Z_CUDA(cudaMemcpy(ws.at<int2>(p->o_tile_desc), tiles.data(), 8ll * tiles.size(), cudaMemcpyHostToDevice));
-	B200Z_CUDA(cudaMemcpy(ws.at<int32_t>(p->o_blk_desc), blk_desc.data(), 4ll * nblk, cudaMemcpyHostToDevice));
-	B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_blk_off), blk_off.data(), 4ll * (n + 1), cudaMemcpyHostToDevice));
-	if (!ck_tiles.empty())
-		B200Z_CUDA(cudaMemcpy(ws.at<CkTile>(p->o_ck_desc), ck_tiles.data(), sizeof(CkTile) * ck_tiles.size(),
-		                      cudaMemcpyHostToDevice));
-	if (lp.func == 2) {
-		if (!chunks.empty())
-			B200Z_CUDA(cudaMemcpy(ws.at<ChunkDesc>(p->o_chunks), chunks.data(), sizeof(ChunkDesc) * chunks.size(), cudaMemcpyHostToDevice));
-		if (!rgroups.empty())
-			B200Z_CUDA(cudaMemcpy(ws.at<int2>(p->o_rgroups), rgroups.data(), 8ll * rgroups.size(), cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_rnd_off), rnd_off.data(), 4ll * (n + 1), cudaMemcpyHostToDevice));
-	}
-	if (lp.func == 1 && n) {
-		if (!sched_flat.empty())
-			B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_sched), sched_flat.data(), 4ll * sched_flat.size(), cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_sched_off), sched_off.data(), 4ll * (n + 1), cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int32_t>(p->o_undrained), undrained32.data(), 4ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<void *>(p->o_fstate), fstate.data(), 8ll * n, cudaMemcpyHostToDevice));
-	}
-	if (!sblocks.empty())
-		B200Z_CUDA(cudaMemcpy(ws.at<StoredBlock>(p->o_stored), sblocks.data(), sizeof(StoredBlock) * sblocks.size(), cudaMemcpyHostToDevice));
-	if (!slens.empty()) B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_slens), slens.data(), 8ll * slens.size(), cudaMemcpyHostToDevice));
 	B200Z_CUDA(cudaFuncSetAttribute(k_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_links, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinksSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileData + 2 * 2 * kTile));
@@ -1762,26 +1762,111 @@ int deflate_plan_build(b200z_plan *p) {
 	return B200Z_OK;
 }
 
-int deflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
+int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strategy, int wrap, int end_mode,
+                        const b200z_history *hist, b200z_plan **out) {
+	std::unique_ptr<DeflatePlan> p(new DeflatePlan());
+	p->device = current_device();
+	p->kind = 0;
+	p->n = n;
+	p->level = level;
+	p->strategy = strategy;
+	p->wrap = wrap;
+	p->end_mode = end_mode;
+	p->in_len.assign(in_len, in_len + n);
+	if (hist && n > 0 && level <= 4) {
+		// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
+		if (hist->chunk_count) {
+			if (!hist->chunk_len) {
+				set_error("history: chunk_count without chunk_len");
+				return B200Z_E_ARG;
+			}
+			p->sched_cum.resize(n);
+			for (int i = 0; i < n; i++) {
+				int64_t sum = 0;
+				for (int k = 0; k < hist->chunk_count[i]; k++) {
+					const int64_t c = hist->chunk_len[i] ? hist->chunk_len[i][k] : -1;
+					if (c < 0) {
+						set_error("stream %d: SetInput size %d", i, k);
+						return B200Z_E_ARG;
+					}
+					sum += c;
+					p->sched_cum[i].push_back((uint32_t)sum);
+				}
+				if (hist->chunk_count[i] < 0 || (hist->chunk_count[i] > 0 && sum != in_len[i])) {
+					set_error("stream %d: the SetInput sizes add up to %lld, the stream has %lld bytes", i, (long long)sum,
+					          (long long)in_len[i]);
+					return B200Z_E_ARG;
+				}
+			}
+		}
+		if (hist->undrained_last) p->undrained.assign(hist->undrained_last, hist->undrained_last + n);
+		if (hist->engine_state && level >= 1) p->engine_state.assign(hist->engine_state, hist->engine_state + n);
+		if (hist->stored_state && level == 0) p->stored_state = hist->stored_state;
+	}
+	if (hist && hist->kind != B200Z_HIST_NONE && n > 0) {
+		if ((hist->kind != B200Z_HIST_DICTIONARY && hist->kind != B200Z_HIST_CONTINUE) || !hist->hist_len) {
+			set_error("history: kind/hist_len");
+			return B200Z_E_ARG;
+		}
+		if (hist->kind == B200Z_HIST_CONTINUE && level < 5) {
+			// DeflateStored / DeflateFast keep window-relative state across Deflate() calls that is not a function of the
+			// stream position: it has to come from the run of the previous segment
+			bool have = level == 0 ? p->stored_state != nullptr : !p->engine_state.empty();
+			for (void *q : p->engine_state) have = have && q != nullptr;
+			if (!have) {
+				set_error("continuing a stream after Flush() at levels 0-4 needs the engine state of the previous segment "
+				          "(b200z_history.engine_state / stored_state)");
+				return B200Z_E_UNSUPPORTED;
+			}
+		}
+		p->hist_kind = hist->kind;
+		p->check_seeded = hist->check_seeded != 0;
+		p->hist.assign(hist->hist_len, hist->hist_len + n);
+		p->pos_base.resize(n);
+		p->bit_base.resize(n);
+		p->hist_mask.resize(n);
+		for (int i = 0; i < n; i++) {
+			const int64_t H = p->hist[i];
+			if (H < 0 || H > 32768 || (hist->kind == B200Z_HIST_DICTIONARY && H > kMaxDist)) {
+				set_error("stream %d: history of %lld bytes (at most %d)", i, (long long)H,
+				          hist->kind == B200Z_HIST_DICTIONARY ? kMaxDist : 32768);
+				return B200Z_E_ARG;
+			}
+			p->pos_base[i] = (hist->pos_base && hist->kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
+			p->bit_base[i] = hist->bit_base ? hist->bit_base[i] : 0;
+			if (p->pos_base[i] < H || p->pos_base[i] > 0xFFFF0000ll || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
+				set_error("stream %d: pos_base/bit_base", i);
+				return B200Z_E_ARG;
+			}
+			if (hist->hist_mask && hist->hist_mask[i]) p->hist_mask[i].assign(hist->hist_mask[i], hist->hist_mask[i] + H);
+			p->in_len[i] += H; // the input slot holds history + data
+		}
+	}
+	const int rc = deflate_plan_build(p.get());
+	if (rc == B200Z_OK) *out = p.release();
+	return rc;
+}
+
+int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_out_bits, cudaStream_t s, int stages) {
+	DeflatePlan *p = static_cast<DeflatePlan *>(plan);
 	const Arena &ws = p->ws;
 	const int n = p->n;
 	if (n == 0) return B200Z_OK;
 	const LevelParams lp = level_params(p->level);
-	const int64_t *in_off = ws.at<int64_t>(p->o_in_off), *in_len = ws.at<int64_t>(p->o_in_len);
-	const int64_t *out_off = ws.at<int64_t>(p->o_out_off), *out_cap = ws.at<int64_t>(p->o_out_cap);
-	uint16_t *link = lp.func == 2 ? ws.at<uint16_t>(p->o_link) : nullptr;
-	uint2 *mt = lp.func == 2 ? ws.at<uint2>(p->o_mt) : nullptr;
-	uint32_t *sym = lp.func != 0 ? ws.at<uint32_t>(p->o_sym) : nullptr;
-	uint32_t *nsyms = ws.at<uint32_t>(p->o_nsyms), *nblocks = ws.at<uint32_t>(p->o_nblocks);
-	uint32_t *blk_off = ws.at<uint32_t>(p->o_blk_off);
-	int32_t *blk_desc = ws.at<int32_t>(p->o_blk_desc);
-	uint32_t *blk_start = ws.at<uint32_t>(p->o_blk_start), *blk_ptop = ws.at<uint32_t>(p->o_blk_ptop);
-	BlockMeta *meta = ws.at<BlockMeta>(p->o_meta);
-	BlockTables *tables = ws.at<BlockTables>(p->o_tables);
-	const uint32_t *hist = ws.at<uint32_t>(p->o_hist), *bit_base = ws.at<uint32_t>(p->o_bitbase);
-	const int64_t *bias = ws.at<int64_t>(p->o_bias);
-	const int ck_fresh = p->check_seeded ? 0 : 1;
+	const int64_t *in_off = ws.at(p->o_in_off), *in_len = ws.at(p->o_in_len);
+	const int64_t *out_off = ws.at(p->o_out_off), *out_cap = ws.at(p->o_out_cap);
+	uint16_t *link = lp.func == 2 ? ws.at(p->o_link) : nullptr;
+	uint2 *mt = lp.func == 2 ? ws.at(p->o_mt) : nullptr;
+	uint32_t *sym = lp.func != 0 ? ws.at(p->o_sym) : nullptr;
+	uint32_t *nsyms = ws.at(p->o_nsyms), *nblocks = ws.at(p->o_nblocks);
+	uint32_t *blk_off = ws.at(p->o_blk_off);
+	int32_t *blk_desc = ws.at(p->o_blk_desc);
+	uint32_t *blk_start = ws.at(p->o_blk_start), *blk_ptop = ws.at(p->o_blk_ptop);
+	BlockMeta *meta = ws.at(p->o_meta);
+	BlockTables *tables = ws.at(p->o_tables);
+	const uint32_t *hist = ws.at(p->o_hist), *bit_base = ws.at(p->o_bitbase);
+	const int64_t *bias = ws.at(p->o_bias);
 
 	// stages: B200Z_STAGE_SEARCH = match finding (levels 5-9: k_links, k_match), B200Z_STAGE_ENCODE = everything else.
 	// Splitting lets a caller put other work (e.g. an inflate plan on a second stream) next to the ENCODE kernels, which
@@ -1799,76 +1884,65 @@ int deflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t
 	if (lp.func == 0) {
 		// level 0: stored blocks laid out when the plan was built
 		p->mark(s, "k_stored");
-		if (p->n_stored) k_stored<<<p->n_stored, 256, 0, s>>>(d_in, d_out, in_off, out_off, ws.at<StoredBlock>(p->o_stored));
-		k_set_results<<<(n + 127) / 128, 128, 0, s>>>(n, ws.at<int64_t>(p->o_slens), d_out_len, d_status, d_out_bits);
-		p->mark(s, "checksum");
-		if (p->wrap != B200Z_WRAP_RAW && d_check) {
-			int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at<int64_t>(p->o_ck_off), ws.at<int64_t>(p->o_ck_len), n,
-			                         ws.at<CkTile>(p->o_ck_desc), p->n_ck_tiles, ws.at<unsigned long long>(p->o_ck_acc), d_check,
-			                         ck_fresh, s);
-			if (rc) return rc;
-		}
-		p->mark(s, "end");
-		B200Z_CUDA(cudaGetLastError());
-		return B200Z_OK;
-	}
-	if (do_encode) {
-		p->mark(s, "memset");
-		B200Z_CUDA(cudaMemsetAsync(d_out, 0, (size_t)p->out_bytes, s));
-	}
-	if (lp.func == 1) {
-		p->mark(s, "k_fast");
-		B200Z_CUDA(cudaMemsetAsync(ws.at<uint32_t>(p->o_fcounter), 0, 4, s));
-		k_fast<<<p->fast_ctas, 32, 2 * p->fast_prev_entries + (p->fast_head_smem ? 65536 : 0), s>>>(
-		    d_in, sym, in_off, in_len, nsyms, nblocks, blk_off, blk_start, blk_ptop, hist, lp, p->strategy, p->end_mode,
-		    p->fast_prev_entries, ws.at<uint32_t>(p->o_sched), ws.at<uint32_t>(p->o_sched_off), ws.at<int32_t>(p->o_undrained),
-		    ws.at<uint8_t *>(p->o_fstate), p->hist_kind == B200Z_HIST_CONTINUE ? 1 : 0, fast_group_enabled(), n,
-		    p->fast_head_smem ? nullptr : ws.at<uint16_t>(p->o_fhead), ws.at<uint32_t>(p->o_fcounter));
+		if (p->n_stored) k_stored<<<p->n_stored, 256, 0, s>>>(d_in, d_out, in_off, out_off, ws.at(p->o_stored));
+		k_set_results<<<(n + 127) / 128, 128, 0, s>>>(n, ws.at(p->o_slens), d_out_len, d_status, d_out_bits);
 	} else {
-		if (do_search) {
-		p->mark(s, "k_links");
-		if (p->n_runs) k_links<<<p->n_runs, kLinkThreads, kLinksSmem, s>>>(d_in, link, in_off, in_len, ws.at<int2>(p->o_run_desc), hist,
-			                                                         ws.at<uint8_t>(p->o_hmask), ws.at<int64_t>(p->o_hm_off), (uint32_t)p->link_run);
-		p->mark(s, "k_match");
-		if (p->n_tiles)
-			k_match<<<p->n_tiles, kMatchThreads, kTileData + 2 * 2 * kTile, s>>>(d_in, link, mt, in_off, in_len,
-			                                                                   ws.at<int2>(p->o_tile_desc), hist, bias, sym, lp);
+		if (do_encode) {
+			p->mark(s, "memset");
+			B200Z_CUDA(cudaMemsetAsync(d_out, 0, (size_t)p->out_bytes, s));
 		}
-		if (!do_encode) {
-			B200Z_CUDA(cudaGetLastError());
-			return B200Z_OK;
-		}
-		p->mark(s, "k_parse");
-		{
-			uint32_t *sym_local = ws.at<uint32_t>(p->o_sym_local);
-			const uint32_t *rnd_off = ws.at<uint32_t>(p->o_rnd_off);
-			RoundRec *recs = ws.at<RoundRec>(p->o_recs);
-			uint32_t *rnd_symoff = ws.at<uint32_t>(p->o_rnd_symoff);
+		if (lp.func == 1) {
+			p->mark(s, "k_fast");
+			B200Z_CUDA(cudaMemsetAsync(ws.at(p->o_fcounter), 0, 4, s));
+			k_fast<<<p->fast_ctas, 32, 2 * p->fast_prev_entries + (p->fast_head_smem ? 65536 : 0), s>>>(
+			    d_in, sym, in_off, in_len, nsyms, nblocks, blk_off, blk_start, blk_ptop, hist, lp, p->strategy, p->end_mode,
+			    p->fast_prev_entries, ws.at(p->o_sched), ws.at(p->o_sched_off), ws.at(p->o_undrained), ws.at(p->o_fstate),
+			    p->hist_kind == B200Z_HIST_CONTINUE ? 1 : 0, fast_group_enabled(), n, p->fast_head_smem ? nullptr : ws.at(p->o_fhead),
+			    ws.at(p->o_fcounter));
+		} else {
+			if (do_search) {
+				p->mark(s, "k_links");
+				if (p->n_runs)
+					k_links<<<p->n_runs, kLinkThreads, kLinksSmem, s>>>(d_in, link, in_off, in_len, ws.at(p->o_run_desc), hist,
+					                                                    ws.at(p->o_hmask), ws.at(p->o_hm_off), (uint32_t)p->link_run);
+				p->mark(s, "k_match");
+				if (p->n_tiles)
+					k_match<<<p->n_tiles, kMatchThreads, kTileData + 2 * 2 * kTile, s>>>(d_in, link, mt, in_off, in_len,
+					                                                                   ws.at(p->o_tile_desc), hist, bias, sym, lp);
+			}
+			if (!do_encode) {
+				B200Z_CUDA(cudaGetLastError());
+				return B200Z_OK;
+			}
+			p->mark(s, "k_parse");
+			uint32_t *sym_local = ws.at(p->o_sym_local);
+			const uint32_t *rnd_off = ws.at(p->o_rnd_off);
+			RoundRec *recs = ws.at(p->o_recs), *ents = ws.at(p->o_ents);
+			uint32_t *rnd_symoff = ws.at(p->o_rnd_symoff);
 			if (p->n_chunks)
-				k_parse_chunk<<<p->n_chunks, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, ws.at<ChunkDesc>(p->o_chunks),
-				                                                 rnd_off, recs, ws.at<RoundRec>(p->o_ents), hist, bias, lp, p->strategy, parse_warm());
-			k_parse_fix<<<n, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, rnd_off, recs, ws.at<RoundRec>(p->o_ents),
-			                                      p->parse_chunk, hist, bias, lp, p->strategy);
+				k_parse_chunk<<<p->n_chunks, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, ws.at(p->o_chunks), rnd_off,
+				                                                 recs, ents, hist, bias, lp, p->strategy, parse_warm());
+			k_parse_fix<<<n, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, rnd_off, recs, ents, p->parse_chunk, hist,
+			                                      bias, lp, p->strategy);
 			k_parse_scan<<<n, 256, 0, s>>>(d_in, in_off, in_len, rnd_off, recs, rnd_symoff, sym, nsyms, nblocks, blk_off, blk_start,
 			                               blk_ptop, hist, p->end_mode);
 			if (p->n_rgroups)
-				k_parse_gather<<<p->n_rgroups, 128, 0, s>>>(sym_local, sym, in_off, in_len, ws.at<int2>(p->o_rgroups), rnd_off, recs,
+				k_parse_gather<<<p->n_rgroups, 128, 0, s>>>(sym_local, sym, in_off, in_len, ws.at(p->o_rgroups), rnd_off, recs,
 				                                           rnd_symoff, blk_off, blk_start, blk_ptop, hist);
 		}
+		p->mark(s, "k_plan");
+		k_plan<<<p->n_blkmax, kPlanThreads, 0, s>>>(sym, in_off, in_len, nsyms, nblocks, blk_off, blk_desc, blk_start, blk_ptop,
+		                                            meta, tables, bias, p->end_mode);
+		p->mark(s, "k_scan");
+		k_scan<<<(n + 127) / 128, 128, 0, s>>>(n, nblocks, blk_off, meta, d_out, out_off, out_cap, d_out_len, d_status,
+		                                       d_out_bits, bit_base, p->end_mode);
+		p->mark(s, "k_emit");
+		k_emit<<<p->n_blkmax, 256, 0, s>>>(d_in, sym, d_out, in_off, out_off, nblocks, blk_off, blk_desc, meta, tables);
 	}
-	p->mark(s, "k_plan");
-	k_plan<<<p->n_blkmax, kPlanThreads, 0, s>>>(sym, in_off, in_len, nsyms, nblocks, blk_off, blk_desc, blk_start, blk_ptop, meta,
-	                                   tables, bias, p->end_mode);
-	p->mark(s, "k_scan");
-	k_scan<<<(n + 127) / 128, 128, 0, s>>>(n, nblocks, blk_off, meta, d_out, out_off, out_cap, d_out_len, d_status,
-	                                       d_out_bits, bit_base, p->end_mode);
-	p->mark(s, "k_emit");
-	k_emit<<<p->n_blkmax, 256, 0, s>>>(d_in, sym, d_out, in_off, out_off, nblocks, blk_off, blk_desc, meta, tables);
 	p->mark(s, "checksum");
 	if (p->wrap != B200Z_WRAP_RAW && d_check) {
-		int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at<int64_t>(p->o_ck_off), ws.at<int64_t>(p->o_ck_len), n,
-		                         ws.at<CkTile>(p->o_ck_desc), p->n_ck_tiles, ws.at<unsigned long long>(p->o_ck_acc), d_check,
-		                         ck_fresh, s);
+		int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at(p->o_ck_off), ws.at(p->o_ck_len), n,
+		                         ws.at(p->o_ck_desc), p->n_ck_tiles, ws.at(p->o_ck_acc), d_check, p->check_seeded ? 0 : 1, s);
 		if (rc) return rc;
 	}
 	p->mark(s, "end");

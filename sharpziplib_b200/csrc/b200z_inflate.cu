@@ -23,6 +23,7 @@
 // reference window holds (trap T13: the reference does not check distances).
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 
 #include <cuda_pipeline.h>
 
@@ -884,13 +885,37 @@ __global__ void k_wrap_tail(const uint8_t *__restrict__ in, const int64_t *__res
 namespace b200z {
 
 // ------------------------------------------------------------------------------------------------
-int inflate_plan_build(b200z_plan *p) {
+struct InflatePlan final : b200z_plan {
+	bool has_start_bits = false; // raw plans: caller-supplied first bit (b200z_inflate_plan_set_start_bits)
+	std::vector<int64_t> comp_off, comp_cap, dict_cap; // where the compressed bytes start in the blob; capacities (b200z_inflate_plan_set_lengths)
+	// block-parallel pipeline (b200z_inflate_par.cuh)
+	bool inf_parallel = true; // false: the serial kernel only (B200Z_INFLATE=serial)
+	uint32_t nwin_total = 0, n_ftiles = 0, fs_cap = 0, round_cap = 0, hdr_cap = 0;
+	int dec1_grid = 0, dec2_grid = 0, find3_grid = 0;
+	int n_ck_tiles = 0;
+	// workspace: per stream the dictionary length, the first deflate bit and the framing's header verdict, and the (bit,
+	// output position) of the last block header reached; then the checksum scratch and the block-parallel pipeline's arrays
+	Slot<uint32_t> o_hist, o_start_bit, o_win_base, o_win_stream, o_cand, o_seg_list, o_match_cap, o_str_nm;
+	Slot<int32_t> o_pre, o_fallback;
+	Slot<int64_t> o_restart, o_mt_off;
+	Slot<unsigned long long> o_ck_acc, o_fs_list;
+	Slot<CkTile> o_ck_desc;
+	Slot<FTile> o_ftiles;
+	Slot<PCounters> o_ctr;
+	Slot<PSeg> o_segs;
+	Slot<PRound> o_rounds;
+	Slot<PBlockHdr> o_hdrs;
+	Slot<MatchTok> o_mlist;
+};
+
+static int inflate_plan_build(InflatePlan *p) {
 	const int n = p->n;
 	p->in_off.resize(n);
 	p->out_off.resize(n);
+	p->comp_off.resize(n);
+	p->comp_cap.resize(n);
 	int64_t io = 0, oo = 0;
 	const bool has_dict = !p->hist.empty();
-	std::vector<int64_t> dev_off(n), dev_len(n);
 	std::vector<uint32_t> dict32(n, 0u);
 	for (int i = 0; i < n; i++) {
 		if (p->in_len[i] < 0 || p->in_len[i] > 0xFFFF0000ll || p->out_cap[i] < 0) {
@@ -901,13 +926,11 @@ int inflate_plan_build(b200z_plan *p) {
 		const int64_t D = has_dict ? p->hist[i] : 0;
 		const int64_t comp = io + align_up(D, 16);
 		p->in_off[i] = comp - D;
-		dev_off[i] = comp;
-		dev_len[i] = p->in_len[i] - D;
-		p->comp_off.push_back(comp);
-		p->comp_cap.push_back(dev_len[i]);
+		p->comp_off[i] = comp;
+		p->comp_cap[i] = p->in_len[i] - D;
 		p->dict_cap.push_back(D);
 		dict32[i] = (uint32_t)D;
-		io = comp + align_up(dev_len[i] + 16, kAlign);
+		io = comp + align_up(p->comp_cap[i] + 16, kAlign);
 		io = align_up(io, kAlign);
 		p->out_off[i] = oo;
 		oo += align_up(p->out_cap[i] + 16, kAlign);
@@ -915,35 +938,32 @@ int inflate_plan_build(b200z_plan *p) {
 	p->in_bytes = io;
 	p->out_bytes = oo;
 	Arena &ws = p->ws;
-	p->o_in_off = ws.reserve(8ll * (n + 1));
-	p->o_in_len = ws.reserve(8ll * (n + 1));
-	p->o_out_off = ws.reserve(8ll * (n + 1));
-	p->o_out_cap = ws.reserve(8ll * (n + 1));
-	p->o_hist = ws.reserve(4ll * (n + 1));
-	p->o_start_bit = ws.reserve(4ll * (n + 1));
-	p->o_pre = ws.reserve(4ll * (n + 1));
-	p->o_restart = ws.reserve(16ll * (n + 1));
-	std::vector<CkTile> ck_tiles;
+	p->upload_streams(p->comp_off, p->comp_cap, 1); // the kernels read the compressed bytes; the dictionary lies in front
+	p->o_hist = ws.upload(dict32, 1);
+	p->o_start_bit = ws.reserve<uint32_t>(n + 1);
+	p->o_pre = ws.reserve<int32_t>(n + 1);
+	p->o_restart = ws.reserve<int64_t>(2ll * (n + 1));
 	if (p->wrap != B200Z_WRAP_RAW) {
 		// checksum of the OUTPUT (Adler-32 for zlib, CRC-32 for gzip and raw+CRC): tiles over the capacities, the kernel takes
 		// the real lengths from d_out_len
+		std::vector<CkTile> ck_tiles;
 		checksum_tiles(p->out_cap.data(), n, ck_tiles, p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, true);
 		p->n_ck_tiles = (int)ck_tiles.size();
-		p->o_ck_desc = ws.reserve((int64_t)sizeof(CkTile) * (ck_tiles.size() + 1));
-		p->o_ck_acc = ws.reserve(16ll * (n + 1));
+		p->o_ck_desc = ws.upload(ck_tiles, 1);
+		p->o_ck_acc = ws.reserve<unsigned long long>(2ll * (n + 1));
 	}
 	// ---- block-parallel pipeline: candidate windows, finder tiles, pools (b200z_inflate_par.cuh) ----
 	{
 		const char *mode = getenv("B200Z_INFLATE");
 		p->inf_parallel = !(mode && strcmp(mode, "serial") == 0);
 	}
-	std::vector<uint32_t> win_base(n + 1, 0u), win_stream, match_cap(n, 0u);
-	std::vector<FTile> ftiles;
-	std::vector<int64_t> mt_off(n, 0);
 	if (p->inf_parallel && n) {
+		std::vector<uint32_t> win_base(n + 1, 0u), win_stream, match_cap(n, 0u);
+		std::vector<FTile> ftiles;
+		std::vector<int64_t> mt_off(n, 0);
 		uint64_t nwin = 0, rounds = 0, bits = 0, mt = 0;
 		for (int i = 0; i < n; i++) {
-			const uint64_t len = (uint64_t)dev_len[i];
+			const uint64_t len = (uint64_t)p->comp_cap[i];
 			win_base[i] = (uint32_t)nwin;
 			const uint64_t w = len ? (len * 8 + kFWMask) >> kFWShift : 1;
 			for (uint64_t k = 0; k < w; k++) win_stream.push_back((uint32_t)i);
@@ -976,42 +996,25 @@ int inflate_plan_build(b200z_plan *p) {
 			p->fs_cap = (uint32_t)(bits / 256 + 1024 > 0x7FFFFFFFull ? 0x7FFFFFFFull : bits / 256 + 1024);
 			p->round_cap = (uint32_t)((rounds + kRoundBatch - 1) / kRoundBatch * kRoundBatch);
 			p->hdr_cap = p->round_cap / kRoundBatch;
-			p->o_win_base = ws.reserve(4ll * (n + 1));
-			p->o_win_stream = ws.reserve(4ll * (int64_t)nwin);
-			p->o_cand = ws.reserve(4ll * (int64_t)nwin);
-			p->o_ftiles = ws.reserve((int64_t)sizeof(FTile) * (int64_t)(ftiles.size() + 1));
-			p->o_fs_list = ws.reserve(8ll * p->fs_cap);
-			p->o_ctr = ws.reserve((int64_t)sizeof(PCounters));
-			p->o_segs = ws.reserve((int64_t)sizeof(PSeg) * (int64_t)(nwin + n));
-			p->o_seg_list = ws.reserve(4ll * (int64_t)(nwin + n));
-			p->o_rounds = ws.reserve((int64_t)sizeof(PRound) * p->round_cap);
-			p->o_hdrs = ws.reserve((int64_t)sizeof(PBlockHdr) * p->hdr_cap);
-			p->o_mlist = ws.reserve((int64_t)sizeof(MatchTok) * (int64_t)mt);
-			p->o_mt_off = ws.reserve(8ll * (n + 1));
-			p->o_match_cap = ws.reserve(4ll * (n + 1));
-			p->o_str_nm = ws.reserve(4ll * (n + 1));
-			p->o_fallback = ws.reserve(4ll * (n + 1));
+			p->o_win_base = ws.upload(win_base);
+			p->o_win_stream = ws.upload(win_stream);
+			p->o_cand = ws.reserve<uint32_t>((int64_t)nwin);
+			p->o_ftiles = ws.upload(ftiles, 1);
+			p->o_fs_list = ws.reserve<unsigned long long>(p->fs_cap);
+			p->o_ctr = ws.reserve<PCounters>(1);
+			p->o_segs = ws.reserve<PSeg>((int64_t)(nwin + n));
+			p->o_seg_list = ws.reserve<uint32_t>((int64_t)(nwin + n));
+			p->o_rounds = ws.reserve<PRound>(p->round_cap);
+			p->o_hdrs = ws.reserve<PBlockHdr>(p->hdr_cap);
+			p->o_mlist = ws.reserve<MatchTok>((int64_t)mt);
+			p->o_mt_off = ws.upload(mt_off, 1);
+			p->o_match_cap = ws.upload(match_cap, 1);
+			p->o_str_nm = ws.reserve<uint32_t>(n + 1);
+			p->o_fallback = ws.reserve<int32_t>(n + 1);
 		}
 	}
 	int rc = ws.alloc();
 	if (rc) return rc;
-	if (n) {
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_in_off), dev_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_in_len), dev_len.data(), 8ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_hist), dict32.data(), 4ll * n, cudaMemcpyHostToDevice));
-		if (!ck_tiles.empty())
-			B200Z_CUDA(cudaMemcpy(ws.at<CkTile>(p->o_ck_desc), ck_tiles.data(), sizeof(CkTile) * ck_tiles.size(), cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_out_off), p->out_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-		B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_out_cap), p->out_cap.data(), 8ll * n, cudaMemcpyHostToDevice));
-		if (p->inf_parallel) {
-			B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_win_base), win_base.data(), 4ll * (n + 1), cudaMemcpyHostToDevice));
-			B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_win_stream), win_stream.data(), 4ll * win_stream.size(), cudaMemcpyHostToDevice));
-			if (!ftiles.empty())
-				B200Z_CUDA(cudaMemcpy(ws.at<FTile>(p->o_ftiles), ftiles.data(), sizeof(FTile) * ftiles.size(), cudaMemcpyHostToDevice));
-			B200Z_CUDA(cudaMemcpy(ws.at<int64_t>(p->o_mt_off), mt_off.data(), 8ll * n, cudaMemcpyHostToDevice));
-			B200Z_CUDA(cudaMemcpy(ws.at<uint32_t>(p->o_match_cap), match_cap.data(), 4ll * n, cudaMemcpyHostToDevice));
-		}
-	}
 	B200Z_CUDA(cudaFuncSetAttribute(k_inflate, cudaFuncAttributeMaxDynamicSharedMemorySize, kInfSmem2));
 	int extra = 0;
 	if (p->inf_parallel && n) {
@@ -1021,9 +1024,8 @@ int inflate_plan_build(b200z_plan *p) {
 		B200Z_CUDA(cudaFuncSetAttribute(k_dec2, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
 		B200Z_CUDA(cudaFuncSetAttribute(k_find, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
 		B200Z_CUDA(cudaFuncSetAttribute(k_find3, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-		int dev = 0, sms = 1, occ1 = 1, occ2 = 1;
-		B200Z_CUDA(cudaGetDevice(&dev));
-		B200Z_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+		int sms = 1, occ1 = 1, occ2 = 1;
+		B200Z_CUDA(sm_count(&sms));
 		B200Z_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ1, k_dec1, kP1Threads, sizeof(Dec1Shared)));
 		B200Z_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, k_dec2, kP1Threads, sizeof(Dec2Shared)));
 		if (occ1 < 1) occ1 = 1;
@@ -1041,13 +1043,81 @@ int inflate_plan_build(b200z_plan *p) {
 	return B200Z_OK;
 }
 
-int inflate_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s) {
+int inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, const int64_t *dict_len,
+                        b200z_plan **out) {
+	std::unique_ptr<InflatePlan> p(new InflatePlan());
+	p->device = current_device();
+	p->kind = 1;
+	p->n = n;
+	p->wrap = wrap;
+	p->in_len.assign(comp_len, comp_len + n);
+	p->out_cap.assign(out_cap, out_cap + n);
+	if (dict_len && n > 0) {
+		p->hist.assign(dict_len, dict_len + n);
+		for (int i = 0; i < n; i++) {
+			if (p->hist[i] < 0 || p->hist[i] > 32768) { // OutputWindow.CopyDict keeps the last WindowSize bytes (:160-166)
+				set_error("stream %d: dictionary of %lld bytes (at most 32768)", i, (long long)p->hist[i]);
+				return B200Z_E_ARG;
+			}
+			p->in_len[i] += p->hist[i];
+		}
+	}
+	const int rc = inflate_plan_build(p.get());
+	if (rc == B200Z_OK) *out = p.release();
+	return rc;
+}
+
+int inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
+	const int rc = p->ws.write(p->o_start_bit, std::vector<uint32_t>(start_bit, start_bit + p->n));
+	if (rc) return rc;
+	p->has_start_bits = true;
+	return B200Z_OK;
+}
+
+int inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, const int64_t *dict_len) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
+	const int n = p->n;
+	std::vector<int64_t> dl(comp_len, comp_len + n);
+	std::vector<uint32_t> d32((size_t)n);
+	for (int i = 0; i < n; i++) {
+		const int64_t D = dict_len ? dict_len[i] : 0;
+		if (comp_len[i] < 0 || comp_len[i] > p->comp_cap[(size_t)i] || D < 0 || D > p->dict_cap[(size_t)i]) {
+			set_error("stream %d: %lld compressed / %lld dictionary bytes exceed what the plan was created for (%lld / %lld)", i,
+			          (long long)comp_len[i], (long long)D, (long long)p->comp_cap[(size_t)i], (long long)p->dict_cap[(size_t)i]);
+			return B200Z_E_ARG;
+		}
+		d32[(size_t)i] = (uint32_t)D;
+	}
+	for (int i = 0; i < n; i++) { // the dictionary ends where the compressed bytes start
+		if (!p->hist.empty()) p->hist[(size_t)i] = d32[(size_t)i];
+		p->in_off[(size_t)i] = p->comp_off[(size_t)i] - d32[(size_t)i];
+		p->in_len[(size_t)i] = comp_len[i] + d32[(size_t)i];
+	}
+	const int rc = p->ws.write(p->o_in_len, dl);
+	return rc ? rc : p->ws.write(p->o_hist, d32);
+}
+
+int inflate_plan_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_pos, cudaStream_t s) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
+	std::vector<int64_t> rp(2 * (size_t)p->n);
+	B200Z_CUDA(cudaMemcpyAsync(rp.data(), p->ws.at(p->o_restart), 16ull * p->n, cudaMemcpyDeviceToHost, s));
+	B200Z_CUDA(cudaStreamSynchronize(s));
+	for (int i = 0; i < p->n; i++) {
+		bit[i] = rp[2 * (size_t)i];
+		out_pos[i] = rp[2 * (size_t)i + 1];
+	}
+	return B200Z_OK;
+}
+
+int inflate_plan_stats(b200z_plan *plan, uint32_t *v, int32_t cap, cudaStream_t s) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
 	uint32_t r[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 	if (p->inf_parallel && p->n) {
 		PCounters c;
 		std::vector<int32_t> fb((size_t)p->n);
-		B200Z_CUDA(cudaMemcpyAsync(&c, p->ws.at<PCounters>(p->o_ctr), sizeof(c), cudaMemcpyDeviceToHost, s));
-		B200Z_CUDA(cudaMemcpyAsync(fb.data(), p->ws.at<int32_t>(p->o_fallback), 4ull * p->n, cudaMemcpyDeviceToHost, s));
+		B200Z_CUDA(cudaMemcpyAsync(&c, p->ws.at(p->o_ctr), sizeof(c), cudaMemcpyDeviceToHost, s));
+		B200Z_CUDA(cudaMemcpyAsync(fb.data(), p->ws.at(p->o_fallback), 4ull * p->n, cudaMemcpyDeviceToHost, s));
 		B200Z_CUDA(cudaStreamSynchronize(s));
 		r[0] = c.fs_count;
 		r[1] = c.nseg;
@@ -1062,8 +1132,9 @@ int inflate_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s) 
 	return B200Z_OK;
 }
 
-int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
+int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_in_used, cudaStream_t s) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
 	const Arena &ws = p->ws;
 	const int n = p->n;
 	if (n == 0) return B200Z_OK;
@@ -1074,46 +1145,46 @@ int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t
 		set_error("inflate plans with framing or checksums need d_check and d_in_used");
 		return B200Z_E_ARG;
 	}
-	const int64_t *in_off = ws.at<int64_t>(p->o_in_off), *in_len = ws.at<int64_t>(p->o_in_len);
-	uint32_t *start_bit = (framed || p->has_start_bits) ? ws.at<uint32_t>(p->o_start_bit) : nullptr;
-	int32_t *pre = framed ? ws.at<int32_t>(p->o_pre) : nullptr;
+	const int64_t *in_off = ws.at(p->o_in_off), *in_len = ws.at(p->o_in_len);
+	uint32_t *start_bit = (framed || p->has_start_bits) ? ws.at(p->o_start_bit) : nullptr;
+	int32_t *pre = framed ? ws.at(p->o_pre) : nullptr;
 	if (framed) {
 		p->mark(s, "k_wrap");
-		k_wrap_head<<<(n + 127) / 128, 128, 0, s>>>(d_in, in_off, in_len, ws.at<uint32_t>(p->o_hist), n, wrap, start_bit, pre);
+		k_wrap_head<<<(n + 127) / 128, 128, 0, s>>>(d_in, in_off, in_len, ws.at(p->o_hist), n, wrap, start_bit, pre);
 	}
-	const uint32_t *dict_len = ws.at<uint32_t>(p->o_hist);
-	const int64_t *out_off = ws.at<int64_t>(p->o_out_off), *out_cap = ws.at<int64_t>(p->o_out_cap);
-	int64_t *restart = ws.at<int64_t>(p->o_restart);
+	const uint32_t *dict_len = ws.at(p->o_hist);
+	const int64_t *out_off = ws.at(p->o_out_off), *out_cap = ws.at(p->o_out_cap);
+	int64_t *restart = ws.at(p->o_restart);
 	const int32_t *only = nullptr;
 	if (p->inf_parallel) {
-		PCounters *ctr = ws.at<PCounters>(p->o_ctr);
-		uint32_t *cand = ws.at<uint32_t>(p->o_cand);
-		const uint32_t *win_base = ws.at<uint32_t>(p->o_win_base);
-		PSeg *segs = ws.at<PSeg>(p->o_segs);
-		uint32_t *seg_list = ws.at<uint32_t>(p->o_seg_list);
-		PRound *rounds = ws.at<PRound>(p->o_rounds);
-		PBlockHdr *hdrs = ws.at<PBlockHdr>(p->o_hdrs);
-		MatchTok *mlist = ws.at<MatchTok>(p->o_mlist);
-		const int64_t *mt_off = ws.at<int64_t>(p->o_mt_off);
-		uint32_t *str_nm = ws.at<uint32_t>(p->o_str_nm);
-		int32_t *fallback = ws.at<int32_t>(p->o_fallback);
-		unsigned long long *fs_list = ws.at<unsigned long long>(p->o_fs_list);
+		PCounters *ctr = ws.at(p->o_ctr);
+		uint32_t *cand = ws.at(p->o_cand);
+		const uint32_t *win_base = ws.at(p->o_win_base);
+		PSeg *segs = ws.at(p->o_segs);
+		uint32_t *seg_list = ws.at(p->o_seg_list);
+		PRound *rounds = ws.at(p->o_rounds);
+		PBlockHdr *hdrs = ws.at(p->o_hdrs);
+		MatchTok *mlist = ws.at(p->o_mlist);
+		const int64_t *mt_off = ws.at(p->o_mt_off);
+		uint32_t *str_nm = ws.at(p->o_str_nm);
+		int32_t *fallback = ws.at(p->o_fallback);
+		unsigned long long *fs_list = ws.at(p->o_fs_list);
 		p->mark(s, "k_find");
 		B200Z_CUDA(cudaMemsetAsync(ctr, 0, sizeof(PCounters), s));
 		B200Z_CUDA(cudaMemsetAsync(cand, 0xFF, 4ull * p->nwin_total, s));
 		if (p->n_ftiles)
-			k_find<<<p->n_ftiles, 256, 0, s>>>(d_in, in_off, in_len, ws.at<FTile>(p->o_ftiles), start_bit, pre, fs_list, ctr, p->fs_cap);
+			k_find<<<p->n_ftiles, 256, 0, s>>>(d_in, in_off, in_len, ws.at(p->o_ftiles), start_bit, pre, fs_list, ctr, p->fs_cap);
 		p->mark(s, "k_find3");
 		k_find3<<<p->find3_grid, 128, 0, s>>>(d_in, in_off, in_len, fs_list, ctr, p->fs_cap, win_base, cand);
 		p->mark(s, "k_seglist");
 		const uint32_t slots = p->nwin_total + (uint32_t)n;
-		k_seglist<<<(slots + 255) / 256, 256, 0, s>>>(n, p->nwin_total, win_base, ws.at<uint32_t>(p->o_win_stream), cand, start_bit, pre, segs,
+		k_seglist<<<(slots + 255) / 256, 256, 0, s>>>(n, p->nwin_total, win_base, ws.at(p->o_win_stream), cand, start_bit, pre, segs,
 		                                            seg_list, ctr);
 		p->mark(s, "k_dec1");
 		k_dec1<<<p->dec1_grid, kP1Threads, sizeof(Dec1Shared), s>>>(d_in, in_off, in_len, segs, seg_list, ctr, win_base, cand, rounds,
 		                                                             p->round_cap, hdrs, p->hdr_cap);
 		p->mark(s, "k_chain");
-		k_chain<<<(n + 127) / 128, 128, 0, s>>>(n, segs, win_base, in_len, out_cap, ws.at<uint32_t>(p->o_match_cap), pre, d_out_len, d_in_used,
+		k_chain<<<(n + 127) / 128, 128, 0, s>>>(n, segs, win_base, in_len, out_cap, ws.at(p->o_match_cap), pre, d_out_len, d_in_used,
 		                                        d_status, restart, str_nm, fallback);
 		p->mark(s, "k_dec2");
 		k_dec2<<<p->dec2_grid, kP1Threads, sizeof(Dec2Shared), s>>>(d_in, d_out, in_off, in_len, out_off, segs, ctr, rounds, p->round_cap, hdrs,
@@ -1127,8 +1198,8 @@ int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t
 	                                           start_bit, pre, restart, only);
 	if (wrap != B200Z_WRAP_RAW) {
 		p->mark(s, "checksum");
-		int rc = checksum_launch(wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_out, ws.at<int64_t>(p->o_out_off), d_out_len, n,
-		                         ws.at<CkTile>(p->o_ck_desc), p->n_ck_tiles, ws.at<unsigned long long>(p->o_ck_acc), d_check, 1, s);
+		int rc = checksum_launch(wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_out, out_off, d_out_len, n, ws.at(p->o_ck_desc), p->n_ck_tiles,
+		                         ws.at(p->o_ck_acc), d_check, 1, s);
 		if (rc) return rc;
 		if (framed) k_wrap_tail<<<(n + 127) / 128, 128, 0, s>>>(d_in, in_off, in_len, n, wrap, d_in_used, d_out_len, d_check, d_status);
 	}

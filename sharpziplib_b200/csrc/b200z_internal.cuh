@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200z.h"
@@ -43,18 +44,43 @@ struct DeviceGuard {
 constexpr int64_t kAlign = 256; // stream slots in the blobs start on 256-byte boundaries (vector loads / bulk copies)
 inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
-// One device allocation carved into typed arrays.
+// The SM count of the calling thread's current device.
+inline cudaError_t sm_count(int *sms) {
+	int dev = 0;
+	const cudaError_t e = cudaGetDevice(&dev);
+	return e == cudaSuccess ? cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) : e;
+}
+
+// An array of T in an Arena.
+template <class T> struct Slot {
+	int64_t off = 0;
+};
+
+// One device allocation carved into typed arrays: a plan reserves and uploads its arrays, then alloc() allocates them all
+// and copies in what upload() was given.
 struct Arena {
 	uint8_t *base = nullptr;
 	int64_t size = 0, used = 0;
-	int64_t reserve(int64_t bytes) { // planning pass: returns offset
-		int64_t off = align_up(used, 256);
-		used = off + bytes;
-		return off;
+	std::vector<std::pair<int64_t, std::vector<uint8_t>>> pending; // (offset, host bytes) that alloc() copies
+	template <class T> Slot<T> reserve(int64_t count) {
+		const int64_t off = align_up(used, 256);
+		used = off + (int64_t)sizeof(T) * count;
+		return Slot<T>{off};
 	}
-	int alloc();
-	void release();
-	template <class T> T *at(int64_t off) const { return reinterpret_cast<T *>(base + off); }
+	// reserves v.size() + spare elements; alloc() fills the first v.size() of them with v
+	template <class T> Slot<T> upload(const std::vector<T> &v, int64_t spare = 0) {
+		const Slot<T> s = reserve<T>((int64_t)v.size() + spare);
+		const uint8_t *b = reinterpret_cast<const uint8_t *>(v.data());
+		pending.emplace_back(s.off, std::vector<uint8_t>(b, b + sizeof(T) * v.size()));
+		return s;
+	}
+	// after alloc(): copies v over the start of the slot
+	template <class T> int write(Slot<T> s, const std::vector<T> &v) {
+		if (!v.empty()) B200Z_CUDA(cudaMemcpy(at(s), v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+		return B200Z_OK;
+	}
+	int alloc(); // the plan that owns the arena frees base
+	template <class T> T *at(Slot<T> s) const { return reinterpret_cast<T *>(base + s.off); }
 };
 
 // per-block tables produced by k_plan and consumed by k_emit
@@ -85,7 +111,13 @@ struct __align__(8) MatchTok {
 
 } // namespace b200z
 
+// What the C-ABI and the host pipelines see of a plan.  Each pipeline derives its plan type from this one, next to its
+// kernels (DeflatePlan in b200z_deflate.cu, InflatePlan in b200z_inflate.cu), and lays out the rest of its workspace there.
 struct b200z_plan {
+	virtual ~b200z_plan() {
+		for (cudaEvent_t e : ev) cudaEventDestroy(e);
+		if (ws.base) cudaFree(ws.base);
+	}
 	int kind = 0; // 0 deflate, 1 inflate
 	int device = -1; // the device the plan's workspace lives on
 	int n = 0;
@@ -95,51 +127,20 @@ struct b200z_plan {
 	int64_t in_bytes = 0, out_bytes = 0;
 	// deflate with history (b200z_deflate_plan_create_ex): in_len[] is history + data; an inflate plan keeps the
 	// preset-dictionary lengths in hist[]
-	int hist_kind = 0; // B200Z_HIST_*
-	bool check_seeded = false;
-	std::vector<int64_t> hist, pos_base;
-	std::vector<int32_t> bit_base;
-	std::vector<std::vector<uint8_t>> hist_mask;
-	int64_t o_hist = 0, o_bias = 0, o_bitbase = 0, o_hm_off = 0, o_hmask = 0, o_ck_off = 0, o_ck_len = 0;
+	std::vector<int64_t> hist;
 	b200z::Arena ws;
+	// per stream on the device: where the kernels find its input and how long it is, where its output goes and how much
+	// room it has (upload_streams)
+	b200z::Slot<int64_t> o_in_off, o_in_len, o_out_off, o_out_cap;
 	int launches = 0;
-	// deflate workspace offsets
-	int64_t o_in_off = 0, o_in_len = 0, o_out_off = 0, o_out_cap = 0;
-	int64_t o_run_desc = 0, o_tile_desc = 0, o_blk_desc = 0, o_blk_off = 0;
-	int64_t o_link = 0, o_mt = 0, o_sym = 0, o_nsyms = 0, o_nblocks = 0;
-	int64_t o_blk_start = 0, o_blk_ptop = 0, o_meta = 0, o_tables = 0;
-	int n_runs = 0, n_tiles = 0, n_blkmax = 0;
-	int64_t o_sym_local = 0, o_chunks = 0, o_rgroups = 0, o_rnd_off = 0, o_recs = 0, o_ents = 0, o_rnd_symoff = 0; // chunked parse
-	int n_chunks = 0, n_rgroups = 0;
-	uint32_t parse_chunk = 32768;
-	int link_run = 65536; // positions per k_links CTA (B200Z_LINK_RUN)
-	int fast_prev_entries = 32768; // k_fast's prev[] size for this batch
-	int fast_ctas = 1;             // k_fast's persistent CTAs (each owns a head[] slot of the pool)
-	bool fast_head_smem = false;   // ... or keeps head[] in shared memory (few streams)
-	int64_t o_stored = 0, o_slens = 0; // level 0: stored-block list and per-stream output lengths
-	// levels 0-4: the SetInput schedule of every stream (cumulative sizes), "Flush()/Finish() behind an undrained SetInput",
-	// and the engine state carried between the segments of a stream (b200z_history)
-	std::vector<std::vector<uint32_t>> sched_cum;
-	std::vector<int32_t> undrained;
-	std::vector<void *> engine_state;             // device pointers (levels 1-4)
-	struct b200z_stored_state *stored_state = nullptr; // caller's host array (level 0), used while the plan is built
-	int64_t o_sched = 0, o_sched_off = 0, o_undrained = 0, o_fstate = 0, o_fhead = 0, o_fcounter = 0;
-	int n_stored = 0;
-	// inflate workspace offsets
-	int64_t o_tok = 0, o_ntok = 0, o_tok_off = 0;
-	int64_t o_start_bit = 0, o_pre = 0; // inflate framing: first deflate bit and header verdict per stream
-	int64_t o_restart = 0;              // inflate: per stream (bit, output position) of the last block header reached
-	bool has_start_bits = false;        // raw inflate plans: caller-supplied first bit (b200z_inflate_plan_set_start_bits)
-	std::vector<int64_t> comp_off, comp_cap, dict_cap; // inflate: where the compressed bytes start in the blob; capacities (b200z_inflate_plan_set_lengths)
-	// inflate, block-parallel pipeline (b200z_inflate_par.cuh)
-	bool inf_parallel = true;           // false: the serial kernel only (B200Z_INFLATE=serial)
-	int64_t o_win_base = 0, o_win_stream = 0, o_cand = 0, o_ftiles = 0, o_fs_list = 0, o_ctr = 0, o_segs = 0, o_seg_list = 0;
-	int64_t o_rounds = 0, o_hdrs = 0, o_mlist = 0, o_mt_off = 0, o_match_cap = 0, o_str_nm = 0, o_fallback = 0;
-	uint32_t nwin_total = 0, n_ftiles = 0, fs_cap = 0, round_cap = 0, hdr_cap = 0;
-	int dec1_grid = 0, dec2_grid = 0, find3_grid = 0;
-	// checksum scratch
-	int64_t o_ck_desc = 0, o_ck_acc = 0;
-	int n_ck_tiles = 0;
+	// reserves the four per-stream tables, each with `spare` unused entries behind the n, and queues their upload
+	void upload_streams(const std::vector<int64_t> &dev_in_off, const std::vector<int64_t> &dev_in_len, int spare) {
+		o_in_off = ws.upload(dev_in_off, spare);
+		o_in_len = ws.upload(dev_in_len, spare);
+		o_out_off = ws.upload(out_off, spare);
+		o_out_cap = ws.upload(out_cap, spare);
+	}
+	const int64_t *dev_out_off() const { return ws.at(o_out_off); }
 	// optional per-kernel timing (b200z_plan_set_timing): events recorded on the run's stream between kernels
 	bool timing = false;
 	std::vector<cudaEvent_t> ev;
@@ -160,11 +161,17 @@ struct b200z_plan {
 };
 
 namespace b200z {
-// implemented in b200z_deflate.cu / b200z_inflate.cu / b200z_checksum.cu
-int deflate_plan_build(b200z_plan *p);
+// implemented in b200z_deflate.cu / b200z_inflate.cu / b200z_checksum.cu; the create functions take arguments the C-ABI
+// has checked and validate the history / dictionary lengths themselves
+int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strategy, int wrap, int end_mode,
+                        const b200z_history *hist, b200z_plan **out);
 int deflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_out_bits, cudaStream_t s, int stages);
-int inflate_plan_build(b200z_plan *p);
+int inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, const int64_t *dict_len,
+                        b200z_plan **out);
+int inflate_plan_set_start_bits(b200z_plan *p, const int32_t *start_bit);
+int inflate_plan_set_lengths(b200z_plan *p, const int64_t *comp_len, const int64_t *dict_len);
+int inflate_plan_restart_points(b200z_plan *p, int64_t *bit, int64_t *out_pos, cudaStream_t s);
 int inflate_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s);
 int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_in_used, cudaStream_t s);
