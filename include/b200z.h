@@ -218,7 +218,7 @@ int32_t b200z_pipeline_in_flight(const b200z_pipeline *pipe); /* batches submitt
 int b200z_pipeline_destroy(b200z_pipeline *pipe);
 
 /* Host-buffer batch calls: one submit + collect on a pipeline of depth 1 that the calling thread keeps for the batch's
- * shape (the last four shapes stay cached: plan, pinned staging and device buffers are not allocated again; 
+ * shape (the last four shapes per device stay cached: plan, pinned staging and device buffers are not allocated again;
  * b200z_release_cached() frees them).  in[i]/out[i] are HOST pointers; status[i] is per stream.  The return value is the
  * first non-OK status, if any. */
 int b200z_deflate_batch(const uint8_t *const *in, const int64_t *in_len, int32_t n, int level, int strategy, int wrap,

@@ -15,6 +15,7 @@
 #include "b200z_internal.cuh"
 
 #include <cstring>
+#include <memory>
 #include <mutex>
 
 namespace b200z {
@@ -499,9 +500,8 @@ using namespace b200z;
 struct b200z_aes_transform {
 	int device = -1, key_bytes = 16, write_mode = 0;
 	uint8_t keys[66];
-	uint8_t *d_keys = nullptr, *d_state = nullptr, *d_buf = nullptr, *d_auth = nullptr;
-	int64_t *d_meta = nullptr; // off, len
-	int64_t cap = 0;
+	DevBuf d_keys, d_state, d_auth, d_meta; // d_meta: off, len
+	DevBuf d_buf;                           // input in the first half, output in the second
 	bool have_auth = false;
 	uint8_t auth[20];
 };
@@ -522,21 +522,20 @@ int b200z_aes_derive_keys(const uint8_t *passwords, const int64_t *pw_off, const
 	rc = crypto_ready();
 	if (rc) return rc;
 	const int64_t pwn = pw_off[n], sn = (int64_t)n * key_bytes / 2, on = (int64_t)n * (2 * key_bytes + 2);
-	uint8_t *d = nullptr;
-	const int64_t o_off = align_up(pwn + 16, 16), o_salt = o_off + 8ll * (n + 1), o_out = align_up(o_salt + sn, 16);
-	B200Z_CUDA(cudaMalloc(&d, (size_t)(o_out + on)));
-	cudaError_t e = cudaSuccess;
-	if (pwn) e = cudaMemcpy(d, passwords, (size_t)pwn, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess) e = cudaMemcpy(d + o_off, pw_off, 8ull * (n + 1), cudaMemcpyHostToDevice);
-	if (e == cudaSuccess) e = cudaMemcpy(d + o_salt, salts, (size_t)sn, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess) {
-		const int nblk = (2 * key_bytes + 2 + 19) / 20;
-		k_pbkdf2<<<(n * nblk + 63) / 64, 64, 0, 0>>>(d, reinterpret_cast<const int64_t *>(d + o_off), d + o_salt, key_bytes, 1000, d + o_out, n);
-		e = cudaGetLastError();
-	}
-	if (e == cudaSuccess) e = cudaMemcpy(keys_out, d + o_out, (size_t)on, cudaMemcpyDeviceToHost);
-	cudaFree(d);
-	if (e != cudaSuccess) return cuda_fail(e, "b200z_aes_derive_keys", __FILE__, __LINE__);
+	Arena lay; // offsets only: the blob is `d`
+	const Slot<uint8_t> o_pw = lay.reserve<uint8_t>(pwn + 16), o_salt = lay.reserve<uint8_t>(sn), o_out = lay.reserve<uint8_t>(on);
+	const Slot<int64_t> o_off = lay.reserve<int64_t>(n + 1);
+	DevBuf d;
+	if ((rc = d.ensure((size_t)lay.used))) return rc;
+	uint8_t *d_pw = d.at(o_pw), *d_salt = d.at(o_salt), *d_out = d.at(o_out);
+	int64_t *d_off = d.at(o_off);
+	if (pwn) B200Z_CUDA(cudaMemcpy(d_pw, passwords, (size_t)pwn, cudaMemcpyHostToDevice));
+	B200Z_CUDA(cudaMemcpy(d_off, pw_off, 8ull * (n + 1), cudaMemcpyHostToDevice));
+	B200Z_CUDA(cudaMemcpy(d_salt, salts, (size_t)sn, cudaMemcpyHostToDevice));
+	const int nblk = (2 * key_bytes + 2 + 19) / 20;
+	k_pbkdf2<<<(n * nblk + 63) / 64, 64, 0, 0>>>(d_pw, d_off, d_salt, key_bytes, 1000, d_out, n);
+	B200Z_CUDA(cudaGetLastError());
+	B200Z_CUDA(cudaMemcpy(keys_out, d_out, (size_t)on, cudaMemcpyDeviceToHost));
 	return B200Z_OK;
 }
 
@@ -578,30 +577,25 @@ int b200z_aes_batch(const uint8_t *const *in, const int64_t *len, int32_t n, int
 		max_len = std::max(max_len, len[i]);
 	}
 	const int64_t kb = (int64_t)n * (2 * key_bytes + 2);
-	const int64_t o_out = align_up(total + 256, 256), o_off = 2 * o_out, o_len = o_off + 8ll * n, o_keys = align_up(o_len + 8ll * n, 256),
-	              o_state = align_up(o_keys + kb, 256), o_auth = o_state + 128ll * n, all = o_auth + 20ll * n;
-	uint8_t *d = nullptr;
-	B200Z_CUDA(cudaMalloc(&d, (size_t)all));
-	cudaError_t e = cudaMemset(d + o_state, 0, 128ull * n);
-	for (int i = 0; i < n && e == cudaSuccess; i++)
-		if (len[i]) e = cudaMemcpyAsync(d + off[i], in[i], (size_t)len[i], cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_off, off.data(), 8ull * n, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_len, len, 8ull * n, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_keys, keys, (size_t)kb, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) {
-		rc = b200z_aes_device(d, d + o_out, reinterpret_cast<const int64_t *>(d + o_off), reinterpret_cast<const int64_t *>(d + o_len), max_len,
-		                      n, key_bytes, d + o_keys, write_mode, d + o_state, 1, d + o_auth, nullptr);
-		if (rc) {
-			cudaFree(d);
-			return rc;
-		}
-		for (int i = 0; i < n && e == cudaSuccess; i++)
-			if (len[i]) e = cudaMemcpyAsync(out[i], d + o_out + off[i], (size_t)len[i], cudaMemcpyDeviceToHost, 0);
-		if (e == cudaSuccess) e = cudaMemcpyAsync(auth, d + o_auth, 20ull * n, cudaMemcpyDeviceToHost, 0);
-		if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-	}
-	cudaFree(d);
-	if (e != cudaSuccess) return cuda_fail(e, "b200z_aes_batch", __FILE__, __LINE__);
+	Arena lay; // offsets only: the blob is `d`
+	const Slot<uint8_t> o_in = lay.reserve<uint8_t>(total + 256), o_out = lay.reserve<uint8_t>(total + 256);
+	const Slot<int64_t> o_off = lay.reserve<int64_t>(n), o_len = lay.reserve<int64_t>(n);
+	const Slot<uint8_t> o_keys = lay.reserve<uint8_t>(kb), o_state = lay.reserve<uint8_t>(128ll * n), o_auth = lay.reserve<uint8_t>(20ll * n);
+	DevBuf d;
+	if ((rc = d.ensure((size_t)lay.used))) return rc;
+	B200Z_CUDA(cudaMemset(d.at(o_state), 0, 128ull * n));
+	for (int i = 0; i < n; i++)
+		if (len[i]) B200Z_CUDA(cudaMemcpyAsync(d.at(o_in) + off[i], in[i], (size_t)len[i], cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_off), off.data(), 8ull * n, cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_len), len, 8ull * n, cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_keys), keys, (size_t)kb, cudaMemcpyHostToDevice, 0));
+	rc = b200z_aes_device(d.at(o_in), d.at(o_out), d.at(o_off), d.at(o_len), max_len, n, key_bytes, d.at(o_keys), write_mode, d.at(o_state), 1,
+	                      d.at(o_auth), nullptr);
+	if (rc) return rc;
+	for (int i = 0; i < n; i++)
+		if (len[i]) B200Z_CUDA(cudaMemcpyAsync(out[i], d.at(o_out) + off[i], (size_t)len[i], cudaMemcpyDeviceToHost, 0));
+	B200Z_CUDA(cudaMemcpyAsync(auth, d.at(o_auth), 20ull * n, cudaMemcpyDeviceToHost, 0));
+	B200Z_CUDA(cudaStreamSynchronize(0));
 	return B200Z_OK;
 }
 
@@ -615,29 +609,19 @@ int b200z_aes_transform_create(const uint8_t *password, int32_t password_len, co
 	*out = nullptr;
 	int rc = check_key_bytes(key_bytes);
 	if (rc) return rc;
-	b200z_aes_transform *t = new b200z_aes_transform();
+	std::unique_ptr<b200z_aes_transform> t(new b200z_aes_transform());
 	t->key_bytes = key_bytes;
 	t->write_mode = write_mode ? 1 : 0;
 	const int64_t pw_off[2] = {0, password_len};
 	rc = b200z_aes_derive_keys(password, pw_off, salt, key_bytes, 1, t->keys);
-	if (rc) {
-		delete t;
-		return rc;
-	}
+	if (rc) return rc;
 	t->device = current_device();
-	t->cap = 1 << 16;
-	cudaError_t e = cudaMalloc(&t->d_keys, 256);
-	if (e == cudaSuccess) e = cudaMalloc(&t->d_state, 128);
-	if (e == cudaSuccess) e = cudaMalloc(&t->d_auth, 32);
-	if (e == cudaSuccess) e = cudaMalloc(&t->d_meta, 16);
-	if (e == cudaSuccess) e = cudaMalloc(&t->d_buf, (size_t)(2 * t->cap));
-	if (e == cudaSuccess) e = cudaMemset(t->d_state, 0, 128);
-	if (e == cudaSuccess) e = cudaMemcpy(t->d_keys, t->keys, (size_t)(2 * key_bytes + 2), cudaMemcpyHostToDevice);
-	if (e != cudaSuccess) {
-		b200z_aes_transform_destroy(t);
-		return cuda_fail(e, "b200z_aes_transform_create", __FILE__, __LINE__);
-	}
-	*out = t;
+	if ((rc = t->d_keys.ensure(256)) || (rc = t->d_state.ensure(128)) || (rc = t->d_auth.ensure(32)) || (rc = t->d_meta.ensure(16)) ||
+	    (rc = t->d_buf.ensure(2 << 16)))
+		return rc;
+	B200Z_CUDA(cudaMemset(t->d_state.p, 0, 128));
+	B200Z_CUDA(cudaMemcpy(t->d_keys.p, t->keys, (size_t)(2 * key_bytes + 2), cudaMemcpyHostToDevice));
+	*out = t.release();
 	return B200Z_OK;
 }
 
@@ -649,21 +633,17 @@ int b200z_aes_transform_block(b200z_aes_transform *t, const uint8_t *in, int64_t
 	}
 	if (count == 0) return B200Z_OK;
 	DeviceGuard g(t->device);
-	if (count > t->cap) {
-		uint8_t *nb = nullptr;
-		const int64_t nc = align_up(count, 65536);
-		B200Z_CUDA(cudaMalloc(&nb, (size_t)(2 * nc)));
-		cudaFree(t->d_buf);
-		t->d_buf = nb;
-		t->cap = nc;
-	}
-	const int64_t meta[2] = {0, count};
-	B200Z_CUDA(cudaMemcpyAsync(t->d_meta, meta, 16, cudaMemcpyHostToDevice, 0));
-	B200Z_CUDA(cudaMemcpyAsync(t->d_buf, in, (size_t)count, cudaMemcpyHostToDevice, 0));
-	int rc = b200z_aes_device(t->d_buf, t->d_buf + t->cap, t->d_meta, t->d_meta + 1, count, 1, t->key_bytes, t->d_keys, t->write_mode, t->d_state,
-	                          0, nullptr, nullptr);
+	int rc = t->d_buf.ensure(2 * (size_t)align_up(count, 65536));
 	if (rc) return rc;
-	B200Z_CUDA(cudaMemcpyAsync(out, t->d_buf + t->cap, (size_t)count, cudaMemcpyDeviceToHost, 0));
+	uint8_t *d_out = t->d_buf.p + t->d_buf.cap / 2;
+	int64_t *d_meta = reinterpret_cast<int64_t *>(t->d_meta.p);
+	const int64_t meta[2] = {0, count};
+	B200Z_CUDA(cudaMemcpyAsync(d_meta, meta, 16, cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(t->d_buf.p, in, (size_t)count, cudaMemcpyHostToDevice, 0));
+	rc = b200z_aes_device(t->d_buf.p, d_out, d_meta, d_meta + 1, count, 1, t->key_bytes, t->d_keys.p, t->write_mode, t->d_state.p, 0, nullptr,
+	                      nullptr);
+	if (rc) return rc;
+	B200Z_CUDA(cudaMemcpyAsync(out, d_out, (size_t)count, cudaMemcpyDeviceToHost, 0));
 	B200Z_CUDA(cudaStreamSynchronize(0));
 	return B200Z_OK;
 }
@@ -686,11 +666,12 @@ int b200z_aes_transform_auth_code(b200z_aes_transform *t, uint8_t *out20) {
 	}
 	if (!t->have_auth) {
 		DeviceGuard g(t->device);
+		int64_t *d_meta = reinterpret_cast<int64_t *>(t->d_meta.p);
 		const int64_t meta[2] = {0, 0};
-		B200Z_CUDA(cudaMemcpyAsync(t->d_meta, meta, 16, cudaMemcpyHostToDevice, 0));
-		k_hmac_sha1<<<1, 64, 0, 0>>>(t->d_buf, t->d_meta, t->d_meta + 1, t->d_keys, t->key_bytes, reinterpret_cast<AesState *>(t->d_state), 1, t->d_auth, 1);
+		B200Z_CUDA(cudaMemcpyAsync(d_meta, meta, 16, cudaMemcpyHostToDevice, 0));
+		k_hmac_sha1<<<1, 64, 0, 0>>>(t->d_buf.p, d_meta, d_meta + 1, t->d_keys.p, t->key_bytes, reinterpret_cast<AesState *>(t->d_state.p), 1, t->d_auth.p, 1);
 		B200Z_CUDA(cudaGetLastError());
-		B200Z_CUDA(cudaMemcpy(t->auth, t->d_auth, 20, cudaMemcpyDeviceToHost));
+		B200Z_CUDA(cudaMemcpy(t->auth, t->d_auth.p, 20, cudaMemcpyDeviceToHost));
 		t->have_auth = true;
 	}
 	memcpy(out20, t->auth, 20);
@@ -700,11 +681,6 @@ int b200z_aes_transform_auth_code(b200z_aes_transform *t, uint8_t *out20) {
 int b200z_aes_transform_destroy(b200z_aes_transform *t) {
 	if (!t) return B200Z_OK;
 	DeviceGuard g(t->device);
-	cudaFree(t->d_keys);
-	cudaFree(t->d_state);
-	cudaFree(t->d_auth);
-	cudaFree(t->d_meta);
-	cudaFree(t->d_buf);
 	delete t;
 	return B200Z_OK;
 }
@@ -789,29 +765,23 @@ int b200z_pkzip_batch(const uint8_t *const *in, const int64_t *len, int32_t n, u
 	std::vector<uint32_t> k(3 * (size_t)n);
 	for (int i = 0; i < 3 * n; i++)
 		k[i] = (uint32_t)keys12[4 * i] | ((uint32_t)keys12[4 * i + 1] << 8) | ((uint32_t)keys12[4 * i + 2] << 16) | ((uint32_t)keys12[4 * i + 3] << 24);
-	const int64_t o_out = align_up(total + 256, 256), o_off = 2 * o_out, o_len = o_off + 8ll * n, o_keys = o_len + 8ll * n, all = o_keys + 12ll * n;
-	uint8_t *d = nullptr;
-	B200Z_CUDA(cudaMalloc(&d, (size_t)all));
-	cudaError_t e = cudaSuccess;
-	for (int i = 0; i < n && e == cudaSuccess; i++)
-		if (len[i]) e = cudaMemcpyAsync(d + off[i], in[i], (size_t)len[i], cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_off, off.data(), 8ull * n, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_len, len, 8ull * n, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_keys, k.data(), 12ull * n, cudaMemcpyHostToDevice, 0);
-	if (e == cudaSuccess) {
-		rc = b200z_pkzip_device(d, d + o_out, reinterpret_cast<const int64_t *>(d + o_off), reinterpret_cast<const int64_t *>(d + o_len), n,
-		                        reinterpret_cast<uint32_t *>(d + o_keys), encrypt, nullptr);
-		if (rc) {
-			cudaFree(d);
-			return rc;
-		}
-		for (int i = 0; i < n && e == cudaSuccess; i++)
-			if (len[i]) e = cudaMemcpyAsync(out[i], d + o_out + off[i], (size_t)len[i], cudaMemcpyDeviceToHost, 0);
-		if (e == cudaSuccess) e = cudaMemcpyAsync(k.data(), d + o_keys, 12ull * n, cudaMemcpyDeviceToHost, 0);
-		if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-	}
-	cudaFree(d);
-	if (e != cudaSuccess) return cuda_fail(e, "b200z_pkzip_batch", __FILE__, __LINE__);
+	Arena lay; // offsets only: the blob is `d`
+	const Slot<uint8_t> o_in = lay.reserve<uint8_t>(total + 256), o_out = lay.reserve<uint8_t>(total + 256);
+	const Slot<int64_t> o_off = lay.reserve<int64_t>(n), o_len = lay.reserve<int64_t>(n);
+	const Slot<uint32_t> o_keys = lay.reserve<uint32_t>(3ll * n);
+	DevBuf d;
+	if ((rc = d.ensure((size_t)lay.used))) return rc;
+	for (int i = 0; i < n; i++)
+		if (len[i]) B200Z_CUDA(cudaMemcpyAsync(d.at(o_in) + off[i], in[i], (size_t)len[i], cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_off), off.data(), 8ull * n, cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_len), len, 8ull * n, cudaMemcpyHostToDevice, 0));
+	B200Z_CUDA(cudaMemcpyAsync(d.at(o_keys), k.data(), 12ull * n, cudaMemcpyHostToDevice, 0));
+	rc = b200z_pkzip_device(d.at(o_in), d.at(o_out), d.at(o_off), d.at(o_len), n, d.at(o_keys), encrypt, nullptr);
+	if (rc) return rc;
+	for (int i = 0; i < n; i++)
+		if (len[i]) B200Z_CUDA(cudaMemcpyAsync(out[i], d.at(o_out) + off[i], (size_t)len[i], cudaMemcpyDeviceToHost, 0));
+	B200Z_CUDA(cudaMemcpyAsync(k.data(), d.at(o_keys), 12ull * n, cudaMemcpyDeviceToHost, 0));
+	B200Z_CUDA(cudaStreamSynchronize(0));
 	for (int i = 0; i < 3 * n; i++)
 		for (int b = 0; b < 4; b++) keys12[4 * i + b] = (uint8_t)(k[i] >> (8 * b));
 	return B200Z_OK;

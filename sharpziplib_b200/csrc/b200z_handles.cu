@@ -1,0 +1,774 @@
+// b200z_handles.cu -- the streaming handles of the C-ABI (include/b200z.h), which mirror Deflater.cs / Inflater.cs member
+// for member.  Each handle runs its plans synchronously from host buffers through one Staging (b200z_host.cuh).
+#include <algorithm>
+#include <cstring>
+
+#include "b200z_host.cuh"
+
+namespace b200z {
+
+// ---- small host helpers ----------------------------------------------------------------------------
+struct HostBits { // carries the sub-byte tail of a flushed stream on the host (PendingBuffer's `bits`, :23-24)
+	uint32_t bits = 0;
+	int count = 0;
+	void put(std::vector<uint8_t> &out, uint32_t v, int n) {
+		bits |= v << count;
+		count += n;
+		while (count >= 8) {
+			out.push_back((uint8_t)bits);
+			bits >>= 8;
+			count -= 8;
+		}
+	}
+	void align(std::vector<uint8_t> &out) {
+		if (count > 0) out.push_back((uint8_t)bits);
+		bits = 0;
+		count = 0;
+	}
+};
+
+void zlib_header(int level, uint8_t h[2], bool preset_dict) { // Deflater.cs:436-464 (trap T11)
+	int header = (8 + (7 << 4)) << 8;
+	int level_flags = (level - 1) >> 1;
+	if (level_flags < 0 || level_flags > 3) level_flags = 3;
+	header |= level_flags << 6;
+	if (preset_dict) header |= 0x20; // DeflaterConstants.PRESET_DICT
+	header += 31 - (header % 31);
+	h[0] = (uint8_t)(header >> 8);
+	h[1] = (uint8_t)header;
+}
+
+const char *inflate_detail_msg(int detail) {
+	switch (detail) {
+	case 1: return "Unknown block type";
+	case 2: return "broken uncompressed block";
+	case 3: return "Illegal rep length code";
+	case 4: return "Illegal rep dist code";
+	case 5: return "Encountered invalid codelength 0";
+	case 6: return "ValueOutOfRangeException: dynamic header code count";
+	case 7: return "Cannot repeat previous code length when no other code length has been read";
+	case 8: return "Cannot repeat code lengths past total number of data code lengths";
+	case 9: return "Inflater dynamic header end-of-block code missing";
+	case 10: return "Code lengths oversubscribed";
+	case 11: return "Adler chksum doesn't match";
+	case 12: return "GZIP crc sum mismatch";
+	case 13: return "Number of bytes mismatch in footer";
+	case 14: return "Error GZIP header, first magic byte doesn't match";
+	case 15: return "Error GZIP header,  second magic byte doesn't match";
+	case 16: return "Error GZIP header, data not in deflate format";
+	case 17: return "Reserved flag bits in GZIP header != 0";
+	case 18: return "Header CRC value mismatch";
+	case 19: return "Header checksum illegal";
+	case 20: return "Compression Method unknown";
+	case 22: return "Needs a preset dictionary";
+	default: return "corrupt deflate data";
+	}
+}
+
+// One run of a handle's single-stream plan on the legacy default stream; returns with the run's metadata in st.h and the
+// produced bytes in st.hout at the stream's out_off.  `in` is the handle's own pageable copy of the input.
+static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const uint32_t *check_seed) {
+	int rc = st.ensure(plan, false);
+	if (!rc) rc = stage_run(plan, st, &in, false, check_seed, 0, 0, nullptr);
+	if (rc) return rc;
+	B200Z_CUDA(cudaStreamSynchronize(0));
+	return streams_down(plan, st, nullptr, 0);
+}
+
+// =====================================================================================================
+// Streaming handles
+// =====================================================================================================
+struct DeflaterH {
+	int level = 6, strategy = 0;
+	bool raw = false;
+	// Deflater.cs state bits (:96-110)
+	bool flushing = false, finishing = false, finished = false;
+	bool header_done = false;
+	bool flushed_once = false; // a sync flush has been emitted and nothing was compressed since
+	// what the engine's window has seen so far, cut to its last 32768 bytes (preset dictionary, then every compressed
+	// segment); hist_mask flags the positions InsertString never saw (the last two of the dictionary / of each segment)
+	std::vector<uint8_t> history, hist_mask;
+	int64_t window_seen = 0;  // dictionary bytes kept + TotalIn: the SlideWindow phase of the next segment
+	bool dict_set = false, deflate_called = false, started = false;
+	uint32_t dict_adler = 0;
+	std::vector<uint8_t> input;    // everything SetInput handed over and not yet compressed
+	std::vector<uint8_t> pending;  // produced bytes not yet drained by Deflate()
+	size_t pending_pos = 0;
+	HostBits tail;                 // sub-byte tail carried between device runs
+	int64_t total_in = 0, total_out = 0;
+	uint32_t adler = 1;
+	// levels 0-4 depend on the call pattern (trap T9) and keep engine state across Flush(): the sizes of the SetInput calls
+	// since the last run, whether Deflate() was called behind the last of them, and what the engines carry
+	std::vector<int64_t> chunks;
+	bool undrained = false;
+	b200z_stored_state sstate = {0, 0, 0, 0}; // level 0 (DeflateStored)
+	DevBuf fstate;                            // levels 1-4 (DeflateFast: head[], prev[], scalars), on the device
+	Staging st;
+};
+
+static void deflater_remember(DeflaterH *d, const uint8_t *seg, size_t len, size_t uninserted) {
+	// append a dictionary/segment to the carried window image
+	d->history.insert(d->history.end(), seg, seg + len);
+	d->hist_mask.insert(d->hist_mask.end(), len, 0);
+	for (size_t k = 0; k < uninserted && k < len; k++) d->hist_mask[d->hist_mask.size() - 1 - k] = 1;
+	if (d->history.size() > 32768) {
+		const size_t cut = d->history.size() - 32768;
+		d->history.erase(d->history.begin(), d->history.begin() + (ptrdiff_t)cut);
+		d->hist_mask.erase(d->hist_mask.begin(), d->hist_mask.begin() + (ptrdiff_t)cut);
+	}
+	d->window_seen += (int64_t)len;
+}
+
+static int deflater_run_device(DeflaterH *d, int end_mode) {
+	// compresses d->input as the next segment of the stream; END_FLUSH keeps the stream open and may end inside a byte
+	const int64_t len = (int64_t)d->input.size();
+	const int64_t H = (int64_t)d->history.size();
+	const bool continuing = d->started; // an earlier segment (possibly empty) has been emitted
+	b200z_history hs;
+	memset(&hs, 0, sizeof hs);
+	const int32_t n_chunks = (int32_t)d->chunks.size();
+	const int64_t *chunk_ptr = d->chunks.data();
+	const int32_t undrained = (d->undrained && n_chunks > 0) ? 1 : 0;
+	void *fstate_ptr = nullptr;
+	if (d->level <= 4) {
+		hs.chunk_count = &n_chunks;
+		hs.chunk_len = &chunk_ptr;
+		hs.undrained_last = &undrained;
+		if (d->level == 0) hs.stored_state = &d->sstate;
+		else {
+			int rc0 = d->fstate.ensure((size_t)b200z_engine_state_bytes());
+			if (rc0) return rc0;
+			fstate_ptr = d->fstate.p;
+			hs.engine_state = &fstate_ptr;
+		}
+	}
+	const int64_t pos_base = d->window_seen;
+	const int32_t bit_base = d->tail.count;
+	const uint8_t *mask = d->hist_mask.data();
+	hs.kind = continuing ? B200Z_HIST_CONTINUE : (H ? B200Z_HIST_DICTIONARY : B200Z_HIST_NONE);
+	hs.check_seeded = 1;
+	hs.hist_len = &H;
+	hs.pos_base = &pos_base;
+	hs.bit_base = &bit_base;
+	hs.hist_mask = &mask;
+	const uint32_t stored_before = d->sstate.input_off;
+	b200z_plan *plan = nullptr;
+	int rc = b200z_deflate_plan_create_ex(1, &len, d->level, d->strategy, d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB, end_mode,
+	                                      (hs.kind != B200Z_HIST_NONE || d->level <= 4) ? &hs : nullptr, &plan);
+	if (rc) return rc;
+	std::vector<uint8_t> slot;
+	const uint8_t *inp = d->input.data();
+	if (H) {
+		slot.reserve((size_t)(H + len));
+		slot.insert(slot.end(), d->history.begin(), d->history.end());
+		slot.insert(slot.end(), d->input.begin(), d->input.end());
+		inp = slot.data();
+	}
+	const uint32_t seed = d->adler; // a plan with history continues the running checksum (hs.check_seeded)
+	rc = handle_run(plan, d->st, inp, (hs.kind != B200Z_HIST_NONE && !d->raw) ? &seed : nullptr);
+	const PipeMeta &r = d->st.h;
+	if (!rc && (r.status[0] & 0xFF) != B200Z_OK) {
+		rc = r.status[0] & 0xFF;
+		set_error("device deflate failed with status %d", rc);
+	}
+	if (!rc) {
+		const uint8_t *o = d->st.hout.p + plan->out_off[0];
+		const int64_t bits = r.in_used[0]; // deflate plans report the exact bit length here (bit_base included)
+		const int64_t whole = bits >> 3;
+		std::vector<uint8_t> seg(o, o + ((bits + 7) >> 3));
+		if (!seg.empty()) seg[0] |= (uint8_t)d->tail.bits; // the carried sub-byte tail completes the first byte
+		d->pending.insert(d->pending.end(), seg.begin(), seg.begin() + (ptrdiff_t)whole);
+		// PendingBuffer keeps the sub-byte tail in `bits` until later writes complete the byte (:168-189)
+		d->tail.count = (int)(bits & 7);
+		d->tail.bits = d->tail.count ? (seg[(size_t)whole] & ((1u << d->tail.count) - 1u)) : 0u;
+		if (end_mode == B200Z_END_FINISH) d->tail.align(d->pending); // FINISHING_STATE: AlignToByte (:507)
+		if (!d->raw) d->adler = r.check[0];
+		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run)
+		d->total_in += d->level == 0 ? (int64_t)(uint32_t)(d->sstate.input_off - stored_before) : len;
+		d->started = true;
+		deflater_remember(d, d->input.data(), (size_t)len, 2);
+		d->input.clear();
+		d->chunks.clear();
+		d->undrained = false;
+	}
+	b200z_plan_destroy(plan);
+	return rc;
+}
+
+// ---- Inflater handle ----------------------------------------------------------------------------------
+// The reference's Inflater is a mode machine that stops at any bit and resumes (Inflater.cs:73-86, :429-552).  The kernel
+// decodes whole plans, so the handle resumes at BLOCK granularity: k_inflate reports the last block header it reached
+// (bit position, output position -- the "restart point"); when more input arrives decoding continues from that header
+// with the last 32 KiB of output in front of it as the window image.  Bytes of a block that was only partly available
+// are decoded again by the next run (they were already delivered; the new run's output replaces them byte for byte).
+// Work is linear in the stream for any SetInput granularity as long as blocks are bounded (the reference's own Deflater
+// cuts a block every 16384 symbols), and the handle holds one block of input / output plus the window, not the stream.
+struct InflaterH {
+	bool raw = false;
+	std::vector<uint8_t> input; // compressed bytes from absolute offset in_base on (what lies in front of the restart point is dropped)
+	int64_t in_base = 0, in_total = 0; // in_total = bytes handed over since Reset = in_base + input.size()
+	bool new_input = false;
+	bool finished = false;
+	bool need_dict = false;
+	bool header_done = false;
+	uint32_t read_adler = 0;   // DICTID from the header (Inflater.readAdler)
+	int64_t raw_off = 0;       // where the raw deflate data starts (behind the zlib header)
+	int64_t rs_bit = 0;        // restart point: bit offset from raw_off of the block header decoding continues at
+	int64_t rs_out = 0;        //                output position of that header
+	std::vector<uint8_t> window; // last <= 32768 bytes of (dictionary ++ output[0, rs_out)): OutputWindow's contents there
+	uint32_t run_adler = 1;    // Adler-32 of output[0, rs_out)
+	std::vector<uint8_t> output; // decoded bytes from output position out_base on (delivered bytes in front of rs_out are dropped)
+	int64_t out_base = 0;
+	int64_t delivered = 0;
+	int64_t consumed = 0; // bytes of input the decoder has used (header + raw + trailer), absolute
+	uint32_t adler = 1;
+	int error = 0;
+	std::string error_msg;
+	Staging st;
+	// one plan per handle, created for capacities and run below them (b200z_inflate_plan_set_lengths): a SetInput + Inflate
+	// pair costs the copies and the kernels, no allocation
+	b200z_plan *plan = nullptr;
+	int64_t plan_comp_cap = 0, plan_out_cap = 0;
+	~InflaterH() { b200z_plan_destroy(plan); }
+	int64_t out_total() const { return out_base + (int64_t)output.size(); }
+};
+
+// decodes from the restart point to the end of what is available; fills output / consumed / finished and moves the
+// restart point forward
+static int inflater_run_device(InflaterH *d) {
+	const int64_t slice_abs = d->raw_off + (d->rs_bit >> 3); // absolute offset of the first compressed byte of this run
+	const int32_t sbit = (int32_t)(d->rs_bit & 7);
+	const int64_t avail = d->in_total - slice_abs;
+	if (avail < 0 || slice_abs < d->in_base) {
+		set_error("inflater restart point outside the kept input");
+		return B200Z_E_INTERNAL;
+	}
+	int64_t cap = avail * 8 + 65536;
+	for (int attempt = 0; attempt < 8; attempt++) {
+		const int64_t D = (int64_t)d->window.size();
+		int rc;
+		if (!d->plan || avail > d->plan_comp_cap || cap > d->plan_out_cap) {
+			b200z_plan_destroy(d->plan);
+			d->plan = nullptr;
+			int64_t cc = 65536;
+			while (cc < avail) cc *= 2;
+			const int64_t oc = std::max(cap, cc * 8 + 65536), dc = 32768;
+			if ((rc = b200z_inflate_plan_create_ex(1, &cc, &oc, B200Z_WRAP_RAW, &dc, &d->plan))) return rc;
+			d->plan_comp_cap = cc;
+			d->plan_out_cap = oc;
+		}
+		b200z_plan *plan = d->plan;
+		if ((rc = b200z_inflate_plan_set_lengths(plan, &avail, &D))) return rc;
+		if ((rc = b200z_inflate_plan_set_start_bits(plan, &sbit))) return rc;
+		const uint8_t *inp = d->input.data() + (slice_abs - d->in_base);
+		std::vector<uint8_t> slot;
+		if (D) { // window image (dictionary, earlier output) directly in front of the compressed bytes
+			slot.reserve((size_t)(D + avail));
+			slot.insert(slot.end(), d->window.begin(), d->window.end());
+			slot.insert(slot.end(), inp, inp + avail);
+			inp = slot.data();
+		}
+		rc = handle_run(plan, d->st, inp, nullptr);
+		const PipeMeta &r = d->st.h;
+		int64_t rbit = 0, rout = 0;
+		if (!rc) rc = b200z_plan_get_restart_points(plan, &rbit, &rout, nullptr);
+		if (rc) return rc;
+		const int st = r.status[0] & 0xFF, detail = (r.status[0] >> 8) & 0xFF;
+		if (st == B200Z_E_NOMEM) {
+			cap = d->plan_out_cap * 8; // (the next attempt makes a larger plan)
+			continue;
+		}
+		// this run's output is output[rs_out, rs_out + out_len): it replaces what an earlier run decoded behind the
+		// restart point (the same bytes, and at least as many)
+		const uint8_t *o = d->st.hout.p + plan->out_off[0];
+		d->output.resize((size_t)(d->rs_out - d->out_base));
+		d->output.insert(d->output.end(), o, o + r.out_len[0]);
+		if (st == B200Z_OK) {
+			d->finished = true;
+			d->consumed = slice_abs + r.in_used[0];
+		} else if (st == B200Z_E_NEED_INPUT) {
+			d->consumed = d->in_total;
+		} else {
+			d->error = st;
+			d->error_msg = inflate_detail_msg(detail);
+			return B200Z_OK;
+		}
+		if (rout < 0 || rout > r.out_len[0] || rbit < sbit || rbit > 8 * avail) {
+			set_error("inflater restart point out of range");
+			return B200Z_E_INTERNAL;
+		}
+		if (rout > 0 || rbit != sbit) {
+			// move the restart point: checksum and window advance over output[rs_out, rs_out + rout)
+			const uint8_t *seg = d->output.data() + (d->rs_out - d->out_base);
+			if (!d->raw && rout > 0 && (rc = b200z_adler32(seg, rout, &d->run_adler))) return rc;
+			if (rout >= 32768) d->window.assign(seg + rout - 32768, seg + rout);
+			else {
+				d->window.insert(d->window.end(), seg, seg + rout);
+				if (d->window.size() > 32768) d->window.erase(d->window.begin(), d->window.end() - 32768);
+			}
+			d->rs_out += rout;
+			d->rs_bit = (d->rs_bit & ~7ll) + rbit;
+		}
+		if (st == B200Z_E_NEED_INPUT) {
+			// compressed bytes in front of the restart point are never looked at again
+			const int64_t keep_from = d->raw_off + (d->rs_bit >> 3);
+			if (keep_from > d->in_base) {
+				d->input.erase(d->input.begin(), d->input.begin() + (keep_from - d->in_base));
+				d->in_base = keep_from;
+			}
+		}
+		return B200Z_OK;
+	}
+	set_error("output larger than any capacity tried");
+	return B200Z_E_NOMEM;
+}
+
+// output in front of both the restart point and the delivery position is not needed any more
+static void inflater_trim_output(InflaterH *d) {
+	const int64_t keep_from = d->delivered < d->rs_out ? d->delivered : d->rs_out;
+	if (keep_from - d->out_base >= 65536) {
+		d->output.erase(d->output.begin(), d->output.begin() + (keep_from - d->out_base));
+		d->out_base = keep_from;
+	}
+}
+
+} // namespace b200z
+
+using namespace b200z;
+
+extern "C" {
+
+int b200z_deflater_create(int level, int raw, void **h) {
+	if (!h) {
+		set_error("h");
+		return B200Z_E_ARG;
+	}
+	if (level == -1) level = 6;
+	else if (level < 0 || level > 9) {
+		set_error("level"); // ArgumentOutOfRangeException(nameof(level)), Deflater.cs:184-187
+		return B200Z_E_ARG;
+	}
+	DeflaterH *d = new DeflaterH();
+	d->level = level;
+	d->raw = raw != 0;
+	*h = d;
+	return B200Z_OK;
+}
+int b200z_deflater_destroy(void *h) {
+	delete (DeflaterH *)h;
+	return B200Z_OK;
+}
+int b200z_deflater_reset(void *h) { // Deflater.Reset :204-210 keeps level and strategy
+	DeflaterH *d = (DeflaterH *)h;
+	d->flushing = d->finishing = d->finished = false;
+	d->header_done = false;
+	d->flushed_once = false;
+	d->input.clear();
+	d->pending.clear();
+	d->pending_pos = 0;
+	d->tail = HostBits();
+	d->total_in = d->total_out = 0;
+	d->adler = 1;
+	d->history.clear();
+	d->hist_mask.clear();
+	d->window_seen = 0;
+	d->dict_set = d->deflate_called = d->started = false;
+	d->dict_adler = 0;
+	d->chunks.clear();
+	d->undrained = false;
+	d->sstate = b200z_stored_state{0, 0, 0, 0};
+	return B200Z_OK;
+}
+int b200z_deflater_set_level(void *h, int level) {
+	DeflaterH *d = (DeflaterH *)h;
+	if (level == -1) level = 6;
+	else if (level < 0 || level > 9) {
+		set_error("level");
+		return B200Z_E_ARG;
+	}
+	if (level != d->level && (!d->input.empty() || d->total_in > 0)) {
+		set_error("SetLevel in mid-stream (DeflaterEngine.SetLevel flushes a block, trap T17) is not accelerated");
+		return B200Z_E_UNSUPPORTED;
+	}
+	d->level = level;
+	return B200Z_OK;
+}
+int b200z_deflater_get_level(void *h, int *level) {
+	*level = ((DeflaterH *)h)->level;
+	return B200Z_OK;
+}
+int b200z_deflater_set_strategy(void *h, int strategy) {
+	if (strategy < 0 || strategy > 2) {
+		set_error("strategy");
+		return B200Z_E_ARG;
+	}
+	DeflaterH *d = (DeflaterH *)h;
+	if (strategy != d->strategy && !d->input.empty()) {
+		// the reference switches at the engine's current strstart (DeflaterEngine.cs:283-298), somewhere inside the input it
+		// holds -- like SetLevel in mid-stream; behind a completed Flush() the switch is exact and allowed
+		set_error("SetStrategy between SetInput and Flush()/Finish() is not accelerated");
+		return B200Z_E_UNSUPPORTED;
+	}
+	d->strategy = strategy;
+	return B200Z_OK;
+}
+int b200z_deflater_set_dictionary(void *h, const uint8_t *dict, int32_t len) {
+	DeflaterH *d = (DeflaterH *)h;
+	// Deflater.SetDictionary :372-381: only in INIT_STATE (before the header went out); the header's FDICT bit and
+	// DICTID come from the engine's Adler-32 over the dictionary, which is then reset (:386-401)
+	if (d->raw || d->deflate_called || d->header_done || d->total_in > 0 || d->dict_set) {
+		// state != INIT_STATE (:561): a raw deflater starts in BUSY_STATE (:206), Deflate() leaves INIT_STATE (:436-464)
+		set_error("SetDictionary: not in the initial state"); // InvalidOperationException
+		return B200Z_E_STATE;
+	}
+	if (len < 0 || (len > 0 && !dict)) {
+		set_error("dictionary/count");
+		return B200Z_E_ARG;
+	}
+	uint32_t a = 1;
+	if (len > 0) {
+		int rc = b200z_adler32(dict, len, &a);
+		if (rc) return rc;
+	}
+	d->dict_adler = a;
+	d->dict_set = true;
+	if (len < kMinMatch) return B200Z_OK; // DeflaterEngine.cs:207-210: too short to matter, not even copied
+	const int32_t keep = len > kMaxDist ? kMaxDist : len; // :212-216
+	deflater_remember(d, dict + (len - keep), (size_t)keep, 2);
+	return B200Z_OK;
+}
+int b200z_deflater_set_input(void *h, const uint8_t *buf, int32_t len) {
+	DeflaterH *d = (DeflaterH *)h;
+	if (d->finishing) {
+		set_error("Finish() already called"); // Deflater.cs:335
+		return B200Z_E_STATE;
+	}
+	if (len < 0 || (len > 0 && !buf)) {
+		set_error("buffer/count");
+		return B200Z_E_ARG;
+	}
+	// one plan slot addresses 4 GiB - 64 KiB (32-bit positions, the window phase included): refuse what could not be
+	// compressed instead of accepting it and failing at Flush() / Finish()
+	if ((int64_t)d->input.size() + len + 32768 > 0xFFFF0000ll || d->window_seen + (int64_t)d->input.size() + len > 0xFFFF0000ll) {
+		set_error("Deflater handle: more than 4 GiB - 64 KiB in one stream (TotalIn %lld, %lld buffered, %d more): use several "
+		          "streams or the batch API",
+		          (long long)d->total_in, (long long)d->input.size(), len);
+		return B200Z_E_UNSUPPORTED;
+	}
+	if (len > 0) d->flushed_once = false;
+	d->input.insert(d->input.end(), buf, buf + len);
+	if (len > 0) {
+		// engine.NeedsInput (DeflaterEngine.cs:187-190) is false until Deflate() has taken the bytes; a zero-length SetInput
+		// leaves it true, so the stream classes do not even call Deflate() for it
+		d->undrained = true;
+		if (d->level <= 4) d->chunks.push_back(len); // the schedule matters for DeflateStored / DeflateFast only (trap T9)
+	}
+	return B200Z_OK;
+}
+int b200z_deflater_flush(void *h) {
+	((DeflaterH *)h)->flushing = true;
+	return B200Z_OK;
+}
+int b200z_deflater_finish(void *h) {
+	DeflaterH *d = (DeflaterH *)h;
+	d->flushing = d->finishing = true;
+	return B200Z_OK;
+}
+
+int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced) {
+	DeflaterH *d = (DeflaterH *)h;
+	if (!produced || cap < 0 || (cap > 0 && !out)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	*produced = 0;
+	d->deflate_called = true;
+	if (!d->flushing && !d->finishing) d->undrained = false; // BUSY_STATE: the engine takes everything SetInput handed over
+	// make output due (Deflater.Deflate :427-522)
+	if (!d->finished && d->pending_pos == d->pending.size() && (d->flushing || d->finishing)) {
+		d->pending.clear();
+		d->pending_pos = 0;
+		if (!d->header_done && !d->raw) {
+			uint8_t hd[2];
+			zlib_header(d->level, hd, d->dict_set);
+			d->pending.push_back(hd[0]);
+			d->pending.push_back(hd[1]);
+			if (d->dict_set) { // DICTID = Adler-32 of the whole dictionary, MSB first (:455-461)
+				for (int sh = 24; sh >= 0; sh -= 8) d->pending.push_back((uint8_t)(d->dict_adler >> sh));
+			}
+		}
+		d->header_done = true;
+		if (d->finishing) {
+			if (d->flushed_once) {
+				// Flush() already emitted every block + the sync padding; Finish adds the final empty block:
+				// levels 1-9 FlushBlock on an empty buffer = static header 011 + EOB 0000000 = value 3 in 10 bits
+				// (DeflaterEngine.cs:750-768); level 0 an empty stored block 01 00 00 FF FF (:614-649)
+				if (d->level == 0) {
+					const uint8_t e5[5] = {1, 0, 0, 0xFF, 0xFF};
+					d->pending.insert(d->pending.end(), e5, e5 + 5);
+				} else {
+					d->tail.put(d->pending, 3, 10);
+					d->tail.align(d->pending);
+				}
+			} else {
+				int rc = deflater_run_device(d, B200Z_END_FINISH);
+				if (rc) return rc;
+			}
+			if (!d->raw) {
+				d->pending.push_back((uint8_t)(d->adler >> 24));
+				d->pending.push_back((uint8_t)(d->adler >> 16));
+				d->pending.push_back((uint8_t)(d->adler >> 8));
+				d->pending.push_back((uint8_t)d->adler);
+			}
+			d->finished = true;
+		} else {
+			// sync flush (level 0 skips the padding, :488)
+			int rc = deflater_run_device(d, B200Z_END_FLUSH);
+			if (rc) return rc;
+			d->flushed_once = true;
+			d->flushing = false;
+		}
+	}
+	size_t avail = d->pending.size() - d->pending_pos;
+	size_t take = avail < (size_t)cap ? avail : (size_t)cap;
+	if (take) memcpy(out, d->pending.data() + d->pending_pos, take);
+	d->pending_pos += take;
+	d->total_out += (int64_t)take;
+	*produced = (int32_t)take;
+	return B200Z_OK;
+}
+int b200z_deflater_needs_input(void *h, int *flag) {
+	// DeflaterEngine.NeedsInput (:187-190): false between SetInput and the Deflate() call that takes the bytes.  The
+	// handle copies on SetInput, but it reports what the reference reports: DeflaterOutputStream.Write calls Deflate()
+	// exactly while this is false (Streams/DeflaterOutputStream.cs:245-275), and whether that call happened before
+	// Flush() / Finish() changes the bytes at levels 0-4 (b200z_history.undrained_last)
+	*flag = ((DeflaterH *)h)->undrained ? 0 : 1;
+	return B200Z_OK;
+}
+int b200z_deflater_is_finished(void *h, int *flag) {
+	DeflaterH *d = (DeflaterH *)h;
+	*flag = (d->finished && d->pending_pos == d->pending.size()) ? 1 : 0; // Deflater.cs:271-277
+	return B200Z_OK;
+}
+int b200z_deflater_total_in(void *h, int64_t *v) {
+	DeflaterH *d = (DeflaterH *)h;
+	*v = d->total_in;
+	return B200Z_OK;
+}
+int b200z_deflater_total_out(void *h, int64_t *v) {
+	*v = ((DeflaterH *)h)->total_out;
+	return B200Z_OK;
+}
+int b200z_deflater_adler(void *h, uint32_t *v) {
+	DeflaterH *d = (DeflaterH *)h;
+	*v = d->raw ? 0u : d->adler;
+	return B200Z_OK;
+}
+
+int b200z_inflater_create(int raw, void **h) {
+	if (!h) {
+		set_error("h");
+		return B200Z_E_ARG;
+	}
+	InflaterH *d = new InflaterH();
+	d->raw = raw != 0;
+	*h = d;
+	return B200Z_OK;
+}
+int b200z_inflater_destroy(void *h) {
+	delete (InflaterH *)h;
+	return B200Z_OK;
+}
+int b200z_inflater_reset(void *h) {
+	InflaterH *d = (InflaterH *)h;
+	d->input.clear();
+	d->output.clear();
+	d->window.clear();
+	d->new_input = d->finished = d->need_dict = d->header_done = false;
+	d->in_base = d->in_total = 0;
+	d->raw_off = 0;
+	d->rs_bit = d->rs_out = 0;
+	d->run_adler = 1;
+	d->out_base = 0;
+	d->delivered = 0;
+	d->consumed = 0;
+	d->adler = 1;
+	d->error = 0;
+	d->read_adler = 0;
+	return B200Z_OK;
+}
+int b200z_inflater_set_dictionary(void *h, const uint8_t *dict, int32_t len) {
+	InflaterH *d = (InflaterH *)h;
+	// Inflater.SetDictionary :589-620
+	if (len < 0 || (len > 0 && !dict)) {
+		set_error("buffer/count");
+		return B200Z_E_ARG;
+	}
+	if (!d->need_dict) {
+		set_error("Dictionary is not needed"); // InvalidOperationException
+		return B200Z_E_STATE;
+	}
+	uint32_t a = 1;
+	if (len > 0) {
+		int rc = b200z_adler32(dict, len, &a);
+		if (rc) return rc;
+	}
+	if (a != d->read_adler) {
+		set_error("Wrong adler checksum"); // SharpZipBaseException
+		return B200Z_E_DATA;
+	}
+	const int32_t keep = len > 32768 ? 32768 : len; // OutputWindow.CopyDict :160-166
+	d->window.assign(dict + (len - keep), dict + len);
+	d->need_dict = false;
+	d->adler = 1;
+	d->new_input = true; // what was handed over behind the header can be decoded now
+	return B200Z_OK;
+}
+int b200z_inflater_set_input(void *h, const uint8_t *buf, int32_t len) {
+	InflaterH *d = (InflaterH *)h;
+	if (len < 0 || (len > 0 && !buf)) {
+		set_error("buffer/count");
+		return B200Z_E_ARG;
+	}
+	if (d->in_total > d->consumed && !d->finished) {
+		set_error("Old input was not completely processed"); // StreamManipulator.cs:263
+		return B200Z_E_STATE;
+	}
+	if (d->finished) {
+		// after the end of the stream the reference keeps unread bytes as RemainingInput; replace them
+		d->input.resize((size_t)(d->consumed - d->in_base));
+		d->in_total = d->consumed;
+	}
+	d->input.insert(d->input.end(), buf, buf + len);
+	d->in_total += len;
+	d->new_input = true;
+	return B200Z_OK;
+}
+
+int b200z_inflater_inflate(void *h, uint8_t *out, int32_t cap, int32_t *produced) {
+	InflaterH *d = (InflaterH *)h;
+	if (!produced || cap < 0 || (cap > 0 && !out)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	*produced = 0;
+	if (d->error) {
+		set_error("%s", d->error_msg.c_str());
+		return d->error;
+	}
+	if (!d->finished && d->new_input) {
+		d->new_input = false;
+		if (!d->raw && !d->header_done) {
+			// (nothing is dropped from `input` before the header is done: in_base == 0 here)
+			if (d->input.size() < 2) {
+				d->consumed = (int64_t)d->input.size();
+				return B200Z_OK; // DecodeHeader needs 16 bits (Inflater.cs:209-215)
+			}
+			const int header = (d->input[0] << 8) | d->input[1];
+			if (header % 31 != 0) {
+				d->error = B200Z_E_DATA;
+				d->error_msg = "Header checksum illegal";
+			} else if ((header & 0x0f00) != (8 << 8)) {
+				d->error = B200Z_E_DATA;
+				d->error_msg = "Compression Method unknown";
+			}
+			if (d->error) {
+				set_error("%s", d->error_msg.c_str());
+				return d->error;
+			}
+			if (header & 0x0020) {
+				// PRESET_DICT: DecodeDict reads the 4-byte DICTID MSB first (:185-203); Inflate() then returns 0 until
+				// SetDictionary supplies a dictionary with that Adler-32
+				if (d->input.size() < 6) {
+					d->consumed = (int64_t)d->input.size();
+					return B200Z_OK;
+				}
+				d->read_adler = ((uint32_t)d->input[2] << 24) | ((uint32_t)d->input[3] << 16) | ((uint32_t)d->input[4] << 8) | d->input[5];
+				d->need_dict = true;
+				d->adler = d->read_adler; // Inflater.Adler reports readAdler while the dictionary is awaited (:823-836)
+				d->header_done = true;
+				d->raw_off = 6;
+				d->consumed = 6;
+				d->new_input = true; // the bytes behind the DICTID wait for SetDictionary
+				return B200Z_OK;
+			}
+			d->header_done = true;
+			d->raw_off = 2;
+		}
+		if (d->need_dict) {
+			d->new_input = true;
+			return B200Z_OK;
+		}
+		int rc = inflater_run_device(d);
+		if (rc) return rc;
+		if (d->finished && !d->raw) {
+			// Adler32 trailer, read MSB first (DecodeChksum :397-418); until it is complete the reference withholds
+			// nothing that was already decoded but is not "finished"
+			if (d->in_total - d->consumed < 4) {
+				d->finished = false;
+				d->consumed = d->in_total;
+				// keep output; the last block is decoded again when the trailer arrives
+			} else {
+				const uint8_t *t = d->input.data() + (d->consumed - d->in_base);
+				const uint32_t want = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
+				uint32_t got = d->run_adler; // output[0, rs_out) is in it already
+				const int64_t rest = d->out_total() - d->rs_out;
+				int rc2 = rest > 0 ? b200z_adler32(d->output.data() + (d->rs_out - d->out_base), rest, &got) : B200Z_OK;
+				if (rc2) return rc2;
+				d->adler = got;
+				if (got != want) {
+					d->error = B200Z_E_DATA;
+					d->error_msg = "Adler chksum doesn't match";
+				}
+				d->consumed += 4;
+			}
+		}
+	}
+	size_t avail = (size_t)(d->out_total() - d->delivered);
+	size_t take = avail < (size_t)cap ? avail : (size_t)cap;
+	if (take) memcpy(out, d->output.data() + (d->delivered - d->out_base), take);
+	d->delivered += (int64_t)take;
+	*produced = (int32_t)take;
+	inflater_trim_output(d);
+	if (take == 0 && d->error) {
+		set_error("%s", d->error_msg.c_str());
+		return d->error;
+	}
+	return B200Z_OK;
+}
+int b200z_inflater_needs_input(void *h, int *flag) {
+	InflaterH *d = (InflaterH *)h;
+	*flag = (d->in_total <= d->consumed) ? 1 : 0; // StreamManipulator.IsNeedingInput
+	return B200Z_OK;
+}
+int b200z_inflater_needs_dictionary(void *h, int *flag) {
+	*flag = ((InflaterH *)h)->need_dict ? 1 : 0; // mode == DECODE_DICT && neededBits == 0 (Inflater.cs:792-798)
+	return B200Z_OK;
+}
+int b200z_inflater_is_finished(void *h, int *flag) {
+	InflaterH *d = (InflaterH *)h;
+	// Inflater.cs:806-812; a trailer that did not verify is an exception from Inflate() in the reference (DecodeChksum
+	// :397-418), so the stream is not "finished" as long as that error has not been delivered
+	*flag = (d->finished && !d->error && d->delivered == d->out_total()) ? 1 : 0;
+	return B200Z_OK;
+}
+int b200z_inflater_remaining_input(void *h, int32_t *v) {
+	InflaterH *d = (InflaterH *)h;
+	*v = (int32_t)(d->in_total - d->consumed);
+	return B200Z_OK;
+}
+int b200z_inflater_total_in(void *h, int64_t *v) {
+	*v = ((InflaterH *)h)->consumed; // totalIn - RemainingInput (Inflater.cs:862-868)
+	return B200Z_OK;
+}
+int b200z_inflater_total_out(void *h, int64_t *v) {
+	*v = ((InflaterH *)h)->delivered;
+	return B200Z_OK;
+}
+int b200z_inflater_adler(void *h, uint32_t *v) {
+	InflaterH *d = (InflaterH *)h;
+	*v = d->raw ? 0u : d->adler;
+	return B200Z_OK;
+}
+
+} // extern "C"

@@ -23,6 +23,7 @@ int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
 
 int ensure_init(); // picks up the current device if b200z_init() was not called explicitly
 int current_device(); // the device b200z_init() chose for the calling thread (the CUDA current device otherwise)
+extern thread_local int t_device; // what b200z_init() chose for the calling thread, -1 before
 
 // Every object (plan, pipeline, handle) remembers the device it was created on; its entry points run there and leave the
 // calling thread's current device as they found it, so that one host thread can drive several GPUs.
@@ -43,6 +44,37 @@ struct DeviceGuard {
 
 constexpr int64_t kAlign = 256; // stream slots in the blobs start on 256-byte boundaries (vector loads / bulk copies)
 inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
+
+template <class T> struct Slot;
+
+// An owned allocation of pinned host (Pinned) or device memory.  ensure() grows it and does not keep the contents.
+template <bool Pinned> struct Buf {
+	uint8_t *p = nullptr;
+	size_t cap = 0;
+	Buf() = default;
+	Buf(Buf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; } // (not copyable)
+	~Buf() { release(); }
+	int ensure(size_t n) {
+		if (n <= cap) return B200Z_OK;
+		release();
+		const cudaError_t e = Pinned ? cudaHostAlloc((void **)&p, n, cudaHostAllocDefault) : cudaMalloc((void **)&p, n);
+		if (e != cudaSuccess) {
+			p = nullptr;
+			set_error("%s of %zu bytes failed: %s", Pinned ? "cudaHostAlloc" : "cudaMalloc", n, cudaGetErrorString(e));
+			return B200Z_E_NOMEM;
+		}
+		cap = n;
+		return B200Z_OK;
+	}
+	void release() {
+		if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+		p = nullptr;
+		cap = 0;
+	}
+	template <class T> T *at(Slot<T> s) const { return reinterpret_cast<T *>(p + s.off); } // a slot an Arena laid out
+};
+using PinnedBuf = Buf<true>;
+using DevBuf = Buf<false>;
 
 // The SM count of the calling thread's current device.
 inline cudaError_t sm_count(int *sms) {
@@ -122,7 +154,6 @@ struct b200z_plan {
 	int device = -1; // the device the plan's workspace lives on
 	int n = 0;
 	int level = 6, strategy = 0, wrap = 0, end_mode = 0;
-	int host_wrap = 0; // the framing the host-buffer pipeline writes around this plan's streams (b200z_pipeline_*)
 	std::vector<int64_t> in_len, in_off, out_off, out_cap;
 	int64_t in_bytes = 0, out_bytes = 0;
 	// deflate with history (b200z_deflate_plan_create_ex): in_len[] is history + data; an inflate plan keeps the

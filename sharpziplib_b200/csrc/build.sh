@@ -6,7 +6,10 @@ NVCC=${NVCC:-nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -diag-suppress 550"
 mkdir -p _build
 pids=()
-for f in b200z_deflate b200z_inflate b200z_checksum b200z_api b200z_crypto; do
+objs=()
+for src in *.cu; do
+  f=${src%.cu}
+  objs+=(_build/$f.o)
   stale=0
   [ -f _build/$f.o ] || stale=1
   for dep in $f.cu *.cuh ../../include/b200z.h build.sh; do
@@ -21,5 +24,5 @@ done
 for pid in "${pids[@]}"; do
   wait "$pid" || { echo "build.sh: a compile failed" >&2; exit 1; }
 done
-$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o ../libb200z.so _build/b200z_deflate.o _build/b200z_inflate.o _build/b200z_checksum.o _build/b200z_api.o _build/b200z_crypto.o
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o ../libb200z.so "${objs[@]}"
 echo built ../libb200z.so

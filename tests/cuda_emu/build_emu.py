@@ -13,7 +13,6 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 # B200Z_EMU_CSRC / B200Z_EMU_OUT: build from another copy of the kernel sources (e.g. one with an experimental patch applied)
 CSRC = os.environ.get("B200Z_EMU_CSRC", os.path.join(ROOT, "sharpziplib_b200", "csrc"))
 OUT = os.environ.get("B200Z_EMU_OUT", os.path.join(HERE, "_build"))
-FILES = ["b200z_deflate.cu", "b200z_inflate.cu", "b200z_checksum.cu", "b200z_api.cu", "b200z_crypto.cu"]
 
 
 def _split_top(s):
@@ -81,14 +80,15 @@ def build(sanitize=False, verbose=False):
     that reads or writes outside its buffers is reported; run python with LD_PRELOAD=libasan and detect_leaks=0)"""
     os.makedirs(os.path.join(OUT, "src"), exist_ok=True)
     so = os.path.join(OUT, "libb200z_emu%s.so" % ("_asan" if sanitize == "asan" else "_san" if sanitize else ""))
-    srcs = [os.path.join(CSRC, f) for f in FILES]
+    files = sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
+    srcs = [os.path.join(CSRC, f) for f in files]
     deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + \
         [os.path.join(HERE, "cuda_emu.h"), os.path.join(HERE, "cuda_emu.cpp"), os.path.abspath(__file__),
          os.path.join(os.path.dirname(os.path.dirname(CSRC)), "include", "b200z.h")]
     if os.path.exists(so) and all(os.path.getmtime(so) >= os.path.getmtime(d) for d in deps):
         return so
     gen = []
-    for f in FILES:
+    for f in files:
         text = open(os.path.join(CSRC, f)).read()
         dst = os.path.join(OUT, "src", f.replace(".cu", ".cpp"))
         # headers are found next to the original sources

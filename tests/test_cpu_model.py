@@ -71,7 +71,7 @@ def test_model_fast_and_stored_levels(model, oracle):
 
 # ---- streams with history: preset dictionary, input after Flush() -------------------------------------------
 class _SegmentedModel:
-    """The bookkeeping of the Deflater handle in b200z_api.cu (carried window image, uninserted-position mask, window
+    """The bookkeeping of the Deflater handle in b200z_handles.cu (carried window image, uninserted-position mask, window
     phase, sub-byte tail), driving the CPU model segment by segment."""
 
     def __init__(self, root, level, strategy=0):

@@ -3,7 +3,7 @@
 `decode_slice` states what k_inflate promises for one stream of a raw plan (sharpziplib_b200/csrc/b200z_inflate.cu): decode
 from bit `start_bit` of the first byte handed over, with `window` as the OutputWindow contents in front of the output;
 report the output, a status, the bytes used, and the RESTART POINT = (bit, output position) of the last block header
-reached.  `ModelInflater` is the handle's algorithm (b200z_api.cu, InflaterH / inflater_run_device) transcribed: it keeps
+reached.  `ModelInflater` is the handle's algorithm (b200z_handles.cu, InflaterH / inflater_run_device) transcribed: it keeps
 only the input behind the restart point, the output behind min(delivered, restart point) and a 32 KiB window image, and
 must deliver exactly the stream's bytes for every SetInput granularity.  The GPU tier runs the same shapes against the
 real kernel and handle (tests/test_gpu_restart.py); this file pins the arithmetic (bit offsets that are not byte
@@ -134,7 +134,7 @@ def decode_slice(data, start_bit=0, window=b""):
 
 
 class ModelInflater:
-    """InflaterH of b200z_api.cu for raw and zlib streams (no preset dictionary)."""
+    """InflaterH of b200z_handles.cu for raw and zlib streams (no preset dictionary)."""
 
     def __init__(self, raw):
         self.raw = raw
