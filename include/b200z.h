@@ -35,7 +35,8 @@ enum { B200Z_STRATEGY_DEFAULT = 0, B200Z_STRATEGY_FILTERED = 1, B200Z_STRATEGY_H
 enum {
 	B200Z_END_FINISH = 0,       /* SetInput* -> Finish()                       (Deflater.cs:262; DeflaterOutputStream.Finish :100) */
 	B200Z_END_FLUSH_FINISH = 1, /* SetInput* -> Flush() -> Finish()            (test pattern InflaterDeflaterTests.cs:49-62)      */
-	B200Z_END_FLUSH = 2         /* SetInput* -> Flush(), stream continues      (Deflater.cs:252, sync padding :486-504)           */
+	B200Z_END_FLUSH = 2,        /* SetInput* -> Flush(), stream continues      (Deflater.cs:252, sync padding :486-504)           */
+	B200Z_END_NONE = 3          /* SetInput* -> Deflate(), stream continues: levels 5-9 plans only, see "open runs" below       */
 };
 
 const char *b200z_last_error(void);
@@ -126,6 +127,30 @@ typedef struct b200z_stored_state { /* DeflateStored's fields between Deflate() 
 	uint32_t slides, input_off;
 } b200z_stored_state;
 int64_t b200z_engine_state_bytes(void);
+
+/* ---- open runs (levels 5-9) -----------------------------------------------------------------------------------
+ * A stream compressed in pieces without Flush(): what Deflate() leaves behind in BUSY_STATE.  Without a flush the
+ * reference's output at levels 5-9 does not depend on how the input arrived (trap T9); blocks end only by the
+ * 16384-symbol rule, and at the end of a block DeflateSlow carries nothing but its parse state.  A B200Z_END_NONE run
+ * parses the loop tops with at least MIN_LOOKAHEAD (262) bytes ahead, writes only the blocks the symbol rule closed
+ * (no final block, no padding; the exact bit length goes to d_in_used) and leaves d_check untouched.  After the run,
+ * get_cut reports per stream the data bytes in front of the first block not written (`covered`: the next run's data
+ * starts there, everything in front of it becomes history, all of it in the hash chains) and the parse state to enter
+ * that run with.  Chaining runs this way, and closing with a Flush / Finish run entered the same way, gives exactly
+ * the bytes of one run over everything.
+ * The entry state (default: a clean start): with prev_available, data byte 0 is the byte the previous run left
+ * pending (trap T10) and the parse goes on at byte 1 with match_len / match_dist, a match found at byte 0 (distance
+ * back from byte 0; only read when match_len >= 3).  Without it match_len is 2. */
+typedef struct b200z_parse_entry {
+	int32_t prev_available; /* 0 or 1 */
+	int32_t match_len;      /* 2, or 3..258 when a match is pending */
+	int64_t match_dist;     /* 1..min(32506, history length) when match_len >= 3, else 0 */
+} b200z_parse_entry;
+/* entry[n]: host array; valid for every end mode of a level 5-9 plan, read by every later run */
+int b200z_deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry);
+/* after a B200Z_END_NONE run: covered[n] and next[n] (host arrays); synchronises `cuda_stream` */
+int b200z_deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, void *cuda_stream);
+
 int b200z_deflate_plan_create_ex(int32_t n, const int64_t *in_len, int level, int strategy, int wrap, int end_mode,
                                  const b200z_history *hist, b200z_plan **plan);
 

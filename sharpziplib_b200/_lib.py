@@ -11,7 +11,7 @@ SO_PATH = os.path.join(_HERE, "libb200z.so")
 
 OK, E_ARG, E_STATE, E_DATA, E_INTERNAL, E_CUDA, E_UNSUPPORTED, E_NOMEM, E_NEED_INPUT = range(9)
 WRAP_RAW, WRAP_ZLIB, WRAP_GZIP, WRAP_RAW_CRC32 = 0, 1, 2, 3
-END_FINISH, END_FLUSH_FINISH, END_FLUSH = 0, 1, 2
+END_FINISH, END_FLUSH_FINISH, END_FLUSH, END_NONE = 0, 1, 2, 3
 
 
 class SharpZipBaseException(Exception):
@@ -79,6 +79,8 @@ _SIGS = {
     "b200z_inflate_plan_set_lengths": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_plan_get_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "b200z_plan_data_offset": (C.c_int64, [C.c_void_p, C.c_int32]),
+    "b200z_deflate_plan_set_entry": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200z_deflate_plan_get_cut": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_plan_destroy": (C.c_int, [C.c_void_p]),
     "b200z_plan_in_bytes": (C.c_int64, [C.c_void_p]),
     "b200z_plan_out_bytes": (C.c_int64, [C.c_void_p]),
@@ -166,6 +168,11 @@ class History(C.Structure):
                 # levels 0-4: SetInput schedule and engine state between segments (NULL = one SetInput, no state)
                 ("chunk_count", C.c_void_p), ("chunk_len", C.c_void_p), ("undrained_last", C.c_void_p),
                 ("engine_state", C.c_void_p), ("stored_state", C.c_void_p)]
+
+
+class ParseEntry(C.Structure):
+    """b200z_parse_entry (include/b200z.h): the parse state an open run of a level 5-9 stream starts from"""
+    _fields_ = [("prev_available", C.c_int32), ("match_len", C.c_int32), ("match_dist", C.c_int64)]
 
 
 def lib():

@@ -70,14 +70,33 @@ class DeflatePlan(_Plan):
     """n independent streams, each what `new Deflater(level, true)` + SetInput(all) + Finish() would produce."""
 
     def __init__(self, in_lens, level=6, strategy=0, wrap=_lib.WRAP_RAW, end_mode=_lib.END_FINISH, dict_lens=None,
-                 chunk_lens=None):
+                 chunk_lens=None, history=None, entry=None):
         """dict_lens: per-stream preset-dictionary bytes (Deflater.SetDictionary; at most 32506, the reference keeps the
         dictionary's tail) stored in the input slot directly in front of the stream's data.
         chunk_lens: per stream, the sizes of the SetInput calls that deliver its data (each followed by Deflate() until
-        IsNeedingInput, as DeflaterOutputStream.Write does); levels 0-4 depend on it (SURVEY.md trap T9), 5-9 ignore it."""
+        IsNeedingInput, as DeflaterOutputStream.Write does); levels 0-4 depend on it (SURVEY.md trap T9), 5-9 ignore it.
+        history: (hist_lens, pos_bases, bit_bases[, masks]) -- levels 5-9, the stream goes on behind earlier runs
+        (B200Z_HIST_CONTINUE); pos_bases are the data's stream offsets, of any size, bit_bases the bits (0..7) the previous
+        run left in its last byte, masks per stream the history positions that are not in the hash chains (default: none,
+        which is what a cut leaves).
+        end_mode=END_NONE (levels 5-9): an open run, see cut().
+        entry: per stream (prev_available, match_len, match_dist), the parse state to start from (set_entry)."""
         lens = np.ascontiguousarray(in_lens, dtype=np.int64)
         h = C.c_void_p()
-        if chunk_lens is not None:
+        if history is not None:
+            hl = np.ascontiguousarray(history[0], dtype=np.int64)
+            pb = np.ascontiguousarray(history[1], dtype=np.int64)
+            bb = np.ascontiguousarray(history[2], dtype=np.int32)
+            assert hl.size == lens.size and pb.size == lens.size and bb.size == lens.size
+            masks = [np.zeros(max(int(x), 1), np.uint8) for x in hl]
+            if len(history) > 3:
+                masks = [np.ascontiguousarray(np.frombuffer(bytes(m) + b"\0", np.uint8)) for m in history[3]]
+            mptrs = (C.c_void_p * lens.size)(*[m.ctypes.data for m in masks])
+            hs = _lib.History(_lib.HIST_CONTINUE, 0, hl.ctypes.data, pb.ctypes.data, bb.ctypes.data, C.addressof(mptrs))
+            _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(lens.size, lens.ctypes.data, level, strategy, wrap, end_mode,
+                                                                  C.addressof(hs), C.byref(h)))
+            self.dict_lens = hl
+        elif chunk_lens is not None:
             assert len(chunk_lens) == lens.size
             arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in chunk_lens]
             counts = np.array([a.size for a in arrs], dtype=np.int32)
@@ -100,6 +119,25 @@ class DeflatePlan(_Plan):
             self.dict_lens = dl
         self.in_lens = lens
         super().__init__(h, lens.size)
+        if entry is not None:
+            self.set_entry(entry)
+
+    def set_entry(self, entry):
+        """per stream (prev_available, match_len, match_dist): the parse state the next runs start from"""
+        assert len(entry) == self.n
+        arr = (_lib.ParseEntry * max(self.n, 1))(*[_lib.ParseEntry(*map(int, e)) for e in entry])
+        _lib.raise_for(_lib.lib().b200z_deflate_plan_set_entry(self._h, arr))
+
+    def cut(self, stream=None):
+        """After an END_NONE run: (covered, entries) -- per stream the data bytes in front of the first block not written
+        (the next run's data starts there) and the (prev_available, match_len, match_dist) to enter that run with.
+        Synchronises the stream."""
+        import torch
+        s = stream if stream is not None else torch.cuda.current_stream()
+        covered = np.zeros(self.n, dtype=np.int64)
+        arr = (_lib.ParseEntry * max(self.n, 1))()
+        _lib.raise_for(_lib.lib().b200z_deflate_plan_get_cut(self._h, covered.ctypes.data, arr, s.cuda_stream))
+        return covered, [(e.prev_available, e.match_len, e.match_dist) for e in arr[:self.n]]
 
 
 class InflatePlan(_Plan):

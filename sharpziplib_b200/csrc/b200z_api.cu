@@ -277,7 +277,7 @@ int b200z_deflate_plan_create_ex(int32_t n, const int64_t *in_len, int level, in
 		set_error("level");
 		return B200Z_E_ARG;
 	}
-	if (strategy < 0 || strategy > 2 || wrap < 0 || wrap > B200Z_WRAP_RAW_CRC32 || end_mode < 0 || end_mode > 2) {
+	if (strategy < 0 || strategy > 2 || wrap < 0 || wrap > B200Z_WRAP_RAW_CRC32 || end_mode < 0 || end_mode > B200Z_END_NONE) {
 		set_error("strategy/wrap/end_mode");
 		return B200Z_E_ARG;
 	}
@@ -285,6 +285,24 @@ int b200z_deflate_plan_create_ex(int32_t n, const int64_t *in_len, int level, in
 	if (rc) return rc;
 	DeviceGuard guard(current_device());
 	return deflate_plan_create(n, in_len, level, strategy, wrap, end_mode, hist, plan);
+}
+
+int b200z_deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry) {
+	DeviceGuard guard(plan ? plan->device : -1);
+	if (!plan || plan->kind != 0 || (plan->n > 0 && !entry)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	return deflate_plan_set_entry(plan, entry);
+}
+
+int b200z_deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, void *cuda_stream) {
+	DeviceGuard guard(plan ? plan->device : -1);
+	if (!plan || plan->kind != 0 || (plan->n > 0 && (!covered || !next))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	return deflate_plan_get_cut(plan, covered, next, (cudaStream_t)cuda_stream);
 }
 
 int b200z_inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, b200z_plan **plan) {

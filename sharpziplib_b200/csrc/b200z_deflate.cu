@@ -438,6 +438,15 @@ __device__ __forceinline__ ParseCarry clean_carry(uint32_t p) {
 struct RoundRec { // what a round leaves behind (5 + 1 words)
 	uint32_t p, mlen, mstart, prevAvail, last_top, cnt;
 };
+// The first loop top a run does not parse.  Finish / Flush parse to the end; an open run (B200Z_END_NONE) stops where
+// DeflateSlow's BUSY_STATE loop stops, at the first loop top with less than MIN_LOOKAHEAD bytes ahead (a match taken at an
+// earlier one may still reach beyond it).  Every top in front of it sees at least 262 bytes, so its match table entries
+// and its step are the same as in a run over more input.
+__device__ __forceinline__ uint32_t parse_end(uint32_t n, int end_mode) {
+	constexpr uint32_t kMinLookahead = kMaxMatch + kMinMatch + 1;
+	if (end_mode != B200Z_END_NONE) return n;
+	return n >= kMinLookahead ? n - (kMinLookahead - 1) : 0u;
+}
 __device__ __forceinline__ ParseCarry rec_carry(const RoundRec &r) {
 	ParseCarry c;
 	c.st.p = r.p;
@@ -449,10 +458,11 @@ __device__ __forceinline__ ParseCarry rec_carry(const RoundRec &r) {
 }
 
 // One round [base, base + kRound) of a stream, entered with `carry` (uniform across the warp; updated to the round's
-// exit state).  The round's symbols go to sround[0 .. cnt).  Returns cnt (uniform).
+// exit state).  Loop tops at or behind `pend` are left alone (parse_end).  The round's symbols go to sround[0 .. cnt).
+// Returns cnt (uniform).
 __device__ __forceinline__ uint32_t parse_round(uint8_t *smem, const uint8_t *data, const uint16_t *lnk, const uint2 *tab,
-                                                uint32_t n, uint32_t H, uint32_t ab, uint32_t base, const LevelParams &lp,
-                                                int strategy, ParseCarry &carry, uint32_t *sround) {
+                                                uint32_t n, uint32_t pend, uint32_t H, uint32_t ab, uint32_t base,
+                                                const LevelParams &lp, int strategy, ParseCarry &carry, uint32_t *sround) {
 	uint2 *s_tab = reinterpret_cast<uint2 *>(smem);
 	uint8_t *s_dat = smem + kParseDatOff; // s_dat[16 + i] = byte at position base + i (16 bytes of history in front)
 	const int lane = threadIdx.x & 31;
@@ -488,7 +498,7 @@ __device__ __forceinline__ uint32_t parse_round(uint8_t *smem, const uint8_t *da
 	ex = entry;
 	uint32_t cnt = 0;
 	bool changed = true;
-	const uint32_t lim = seg_end < n ? seg_end : n;
+	const uint32_t lim = seg_end < pend ? seg_end : pend;
 	for (int it = 0; it < 34; it++) {
 		// all lanes step together and re-converge every iteration (a per-lane loop would leave them diverged)
 		if (changed) {
@@ -541,20 +551,21 @@ __global__ void __launch_bounds__(32)
     k_parse_chunk(const uint8_t *__restrict__ in, const uint16_t *__restrict__ link, const uint2 *__restrict__ mt,
                   uint32_t *__restrict__ sym_local, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len,
                   const ChunkDesc *__restrict__ chunks, const uint32_t *__restrict__ rnd_off, RoundRec *__restrict__ recs,
-                  RoundRec *__restrict__ ents, const uint32_t *__restrict__ hist, const int64_t *__restrict__ bias, LevelParams lp,
-                  int strategy, int warm) {
+                  RoundRec *__restrict__ ents, const uint32_t *__restrict__ hist, const int64_t *__restrict__ bias,
+                  const RoundRec *__restrict__ entry, LevelParams lp, int strategy, int warm, int end_mode) {
 	extern __shared__ __align__(16) uint8_t smem[];
 	const ChunkDesc cd = chunks[blockIdx.x];
 	const uint32_t n = (uint32_t)in_len[cd.stream];
+	const uint32_t pend = parse_end(n, end_mode);
 	const int64_t off = in_off[cd.stream];
 	RoundRec *rr = recs + rnd_off[cd.stream];
 	const uint32_t H = hist[cd.stream], ab = (uint32_t)bias[cd.stream];
-	// exact for the first chunk (DeflaterEngine.Reset :234-253; also the state right after a dictionary or a flush).  Every
-	// other chunk parses kParseWarm positions in front of its first one from a clean state (lane 0, straight from global
-	// memory): DeflateSlow's state re-synchronises within a few symbols, so the state this reaches at c0 is the true one at
-	// 99.8 % of the boundaries (tools/tile_fixup.cpp).  It is recorded; k_parse_fix compares it with the exit of the chunk in
-	// front and parses again only where they differ.
-	ParseCarry carry = clean_carry(cd.c0 > H ? cd.c0 : H);
+	// exact for the first chunk: the stream's entry state (DeflaterEngine.Reset :234-253, the state right after a dictionary
+	// or a flush, or what an open run left at its cut).  Every other chunk parses kParseWarm positions in front of its first
+	// one from a clean state (lane 0, straight from global memory): DeflateSlow's state re-synchronises within a few symbols,
+	// so the state this reaches at c0 is the true one at 99.8 % of the boundaries (tools/tile_fixup.cpp).  It is recorded;
+	// k_parse_fix compares it with the exit of the chunk in front and parses again only where they differ.
+	ParseCarry carry = cd.c0 == 0 ? rec_carry(entry[cd.stream]) : clean_carry(cd.c0 > H ? cd.c0 : H);
 	if (cd.c0 > H && warm > 0) {
 		if (threadIdx.x == 0) {
 			const uint8_t *data = in + off;
@@ -589,7 +600,7 @@ __global__ void __launch_bounds__(32)
 		ents[rnd_off[cd.stream] + cd.c0 / kRound] = e;
 	}
 	for (uint32_t base = cd.c0; base < cd.c1; base += kRound) {
-		const uint32_t cnt = parse_round(smem, in + off, link + off, mt + off, n, H, ab, base, lp, strategy, carry, sym_local + off + base);
+		const uint32_t cnt = parse_round(smem, in + off, link + off, mt + off, n, pend, H, ab, base, lp, strategy, carry, sym_local + off + base);
 		if (threadIdx.x == 0) {
 			RoundRec r;
 			r.p = carry.st.p;
@@ -607,10 +618,11 @@ __global__ void __launch_bounds__(32)
     k_parse_fix(const uint8_t *__restrict__ in, const uint16_t *__restrict__ link, const uint2 *__restrict__ mt,
                 uint32_t *__restrict__ sym_local, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len,
                 const uint32_t *__restrict__ rnd_off, RoundRec *__restrict__ recs, const RoundRec *__restrict__ ents, uint32_t chunk,
-                const uint32_t *__restrict__ hist, const int64_t *__restrict__ bias, LevelParams lp, int strategy) {
+                const uint32_t *__restrict__ hist, const int64_t *__restrict__ bias, LevelParams lp, int strategy, int end_mode) {
 	extern __shared__ __align__(16) uint8_t smem[];
 	const int stream = blockIdx.x;
 	const uint32_t n = (uint32_t)in_len[stream];
+	const uint32_t pend = parse_end(n, end_mode);
 	if (n <= chunk) return; // a single chunk was parsed from the true initial state
 	const int64_t off = in_off[stream];
 	RoundRec *rr = recs + rnd_off[stream];
@@ -643,7 +655,8 @@ __global__ void __launch_bounds__(32)
 		ParseCarry truth = rec_carry(rr[c0 / kRound - 1]);
 		for (uint32_t base = c0; base < c1; base += kRound) {
 			const ParseCarry old_exit = rec_carry(rr[base / kRound]);
-			const uint32_t cnt = parse_round(smem, in + off, link + off, mt + off, n, H, ab, base, lp, strategy, truth, sym_local + off + base);
+			const uint32_t cnt = parse_round(smem, in + off, link + off, mt + off, n, pend, H, ab, base, lp, strategy, truth,
+			                                 sym_local + off + base);
 			__syncwarp();
 			if (lane == 0) {
 				RoundRec r;
@@ -706,7 +719,8 @@ __global__ void __launch_bounds__(256)
 		bstart[0] = H;
 		uint32_t nblk = total >> 14;
 		const bool ended_full = end_mode == B200Z_END_FINISH && total > 0 && (total & (uint32_t)(kBlockSyms - 1)) == 0 && !fin.st.prevAvail;
-		if (!ended_full) {
+		// an open run writes the blocks the symbol rule closed and nothing else: the rest is parsed again by the next run
+		if (!ended_full && end_mode != B200Z_END_NONE) {
 			// final flush at lookahead == 0 (DeflaterEngine.cs:750-768)
 			if (fin.st.prevAvail) (sym + in_off[stream])[total++] = sym_lit(in[in_off[stream] + fin.st.p - 1]);
 			bptop[nblk] = fin.last_top;
@@ -761,6 +775,59 @@ __global__ void __launch_bounds__(128)
 			}
 		}
 	}
+}
+
+// Open runs (B200Z_END_NONE): the parse state right behind the last block cut, i.e. behind the tally of symbol K - 1 with
+// K = nblocks * 16384, which the next run of the stream is entered with (its byte `p - prevAvail` is the first one not
+// written).  The rounds only record their exit states, so the round holding symbol K - 1 is parsed again from its entry up
+// to the cut: at most one round of loop tops, one thread per stream.  Without a cut the entry stands.
+__global__ void k_parse_cut(const uint8_t *__restrict__ in, const uint16_t *__restrict__ link, const uint2 *__restrict__ mt,
+                            const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len, const uint32_t *__restrict__ rnd_off,
+                            const RoundRec *__restrict__ recs, const uint32_t *__restrict__ rnd_symoff,
+                            const uint32_t *__restrict__ nblocks, const int64_t *__restrict__ bias, const RoundRec *__restrict__ entry,
+                            RoundRec *__restrict__ cut, int nstreams, LevelParams lp, int strategy) {
+	const int stream = blockIdx.x * blockDim.x + threadIdx.x;
+	if (stream >= nstreams) return;
+	const uint32_t n = (uint32_t)in_len[stream];
+	const uint32_t K = nblocks[stream] * (uint32_t)kBlockSyms;
+	ParseCarry c = rec_carry(entry[stream]);
+	if (K > 0) {
+		const int64_t off = in_off[stream];
+		const uint8_t *data = in + off;
+		const uint16_t *lnk = link + off;
+		const uint2 *tab = mt + off;
+		const uint32_t ab = (uint32_t)bias[stream];
+		const uint32_t *so = rnd_symoff + rnd_off[stream];
+		const RoundRec *rr = recs + rnd_off[stream];
+		// the last round whose first symbol comes before K holds symbol K - 1 (symbol offsets never decrease)
+		uint32_t lo = 0, hi = (n + kRound - 1) / kRound - 1;
+		while (lo < hi) {
+			const uint32_t mid = (lo + hi + 1) >> 1;
+			if (so[mid] < K) lo = mid;
+			else hi = mid - 1;
+		}
+		if (lo > 0) c = rec_carry(rr[lo - 1]);
+		auto tabg = [&](uint32_t p, uint32_t &a, uint32_t &b) {
+			const uint2 t = tab[p];
+			a = t.x;
+			b = t.y;
+		};
+		auto byteg = [&](uint32_t q) { return (uint32_t)data[q]; };
+		auto slowg = [&](uint32_t p, uint32_t m0, uint32_t budget) { return match_search_above(data, lnk, p, n, m0, budget, ab); };
+		for (uint32_t k = so[lo]; k < K;) {
+			c.last_top = c.st.p;
+			uint32_t s2;
+			k += (uint32_t)parse_step(c.st, n, lp, strategy, tabg, byteg, slowg, s2);
+		}
+	}
+	RoundRec r;
+	r.p = c.st.p;
+	r.mlen = c.st.mlen;
+	r.mstart = c.st.mstart;
+	r.prevAvail = c.st.prevAvail;
+	r.last_top = c.last_top;
+	r.cnt = K;
+	cut[stream] = r;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1310,7 +1377,8 @@ __global__ void __launch_bounds__(kPlanThreads)
 		const uint32_t *bptop = blk_ptop + blk_off[stream];
 		const uint32_t byte_start = bstart[b];
 		const uint32_t n = (uint32_t)in_len[stream];
-		const uint32_t byte_len = (b + 1 < nb ? bstart[b + 1] : n) - byte_start;
+		// (an open run's last written block ends at a cut, like every block in front of it)
+		const uint32_t byte_len = ((b + 1 < nb || end_mode == B200Z_END_NONE) ? bstart[b + 1] : n) - byte_start;
 		// storedOffset is window relative and goes negative once the block start has been slid out (trap T4)
 		const long long ab = bias[stream]; // absolute stream offset of buffer position 0
 		long long storedOffset = (long long)byte_start + ab + 1 - 32768ll * (long long)slides_done((uint32_t)(bptop[b] + ab));
@@ -1368,7 +1436,7 @@ __global__ void k_scan(int nstreams, const uint32_t *__restrict__ nblocks, const
 	}
 	uint64_t tail0 = cur;
 	int ntail10 = 0; // number of 10-bit empty static blocks: "WriteBits(2, 10)" (Deflater.cs:486-504)
-	if (end_mode != B200Z_END_FINISH) {
+	if (end_mode == B200Z_END_FLUSH || end_mode == B200Z_END_FLUSH_FINISH) {
 		int neededbits = 8 + (int)((0 - cur) & 7);
 		while (neededbits > 0) {
 			++ntail10;
@@ -1522,6 +1590,9 @@ struct DeflatePlan final : b200z_plan {
 	Slot<uint32_t> o_sym_local, o_rnd_off, o_rnd_symoff;
 	Slot<ChunkDesc> o_chunks;
 	Slot<RoundRec> o_recs, o_ents;
+	Slot<RoundRec> o_entry, o_cut; // per stream: the parse state a run starts from, and where an open run stopped
+	std::vector<RoundRec> entry;   // what o_entry holds (b200z_deflate_plan_set_entry; a clean start by default)
+	bool cut_ready = false;        // an open run has been launched since the plan was made
 	Slot<StoredBlock> o_stored; // level 0
 	Slot<int64_t> o_slens;
 	Slot<uint32_t> o_sched, o_sched_off, o_fcounter; // levels 1-4
@@ -1708,6 +1779,10 @@ static int deflate_plan_build(DeflatePlan *p) {
 		p->o_recs = ws.reserve<RoundRec>(nrounds + 1);
 		p->o_ents = ws.reserve<RoundRec>(nrounds + 1);
 		p->o_rnd_symoff = ws.reserve<uint32_t>(nrounds + 1);
+		p->entry.resize(n);
+		for (int i = 0; i < n; i++) p->entry[i] = RoundRec{hist32[i], (uint32_t)kMinMatch - 1, 0u, 0u, hist32[i], 0u};
+		p->o_entry = ws.upload(p->entry, 1);
+		p->o_cut = ws.reserve<RoundRec>(n + 1);
 	}
 	if (lp.func != 0) p->o_sym = ws.reserve<uint32_t>(io + 16);
 	if (lp.func == 0) {
@@ -1759,6 +1834,7 @@ static int deflate_plan_build(DeflatePlan *p) {
 	B200Z_CUDA(cudaFuncSetAttribute(k_links, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinksSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileData + 2 * 2 * kTile));
 	p->launches = (lp.func == 2 ? 9 : (lp.func == 1 ? 4 : 2)) + (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // + one memset node
+	if (p->end_mode == B200Z_END_NONE) p->launches += 1 - (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // k_parse_cut, no checksum
 	return B200Z_OK;
 }
 
@@ -1773,6 +1849,12 @@ int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strateg
 	p->wrap = wrap;
 	p->end_mode = end_mode;
 	p->in_len.assign(in_len, in_len + n);
+	if (end_mode == B200Z_END_NONE && level <= 4) {
+		// DeflateStored / DeflateFast carry window-relative tables across Deflate() calls that depend on the parse: a run
+		// cannot be resumed from a parse state alone
+		set_error("open runs (B200Z_END_NONE) are for levels 5-9");
+		return B200Z_E_UNSUPPORTED;
+	}
 	if (hist && n > 0 && level <= 4) {
 		// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
 		if (hist->chunk_count) {
@@ -1834,8 +1916,18 @@ int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strateg
 			}
 			p->pos_base[i] = (hist->pos_base && hist->kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
 			p->bit_base[i] = hist->bit_base ? hist->bit_base[i] : 0;
-			if (p->pos_base[i] < H || p->pos_base[i] > 0xFFFF0000ll || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
+			if (p->pos_base[i] < H || (level <= 4 && p->pos_base[i] > 0xFFFF0000ll) || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
 				set_error("stream %d: pos_base/bit_base", i);
+				return B200Z_E_ARG;
+			}
+			// Levels 5-9 read the position only through the window phase, which is periodic with 32768 from kSlideFirst on
+			// (is_slide_pos, slides_done; storedOffset moves with both): the equal phase in the first period keeps the
+			// kernels' 32-bit positions valid in a stream of any length
+			if (level >= 5 && p->pos_base[i] >= (int64_t)kSlideFirst)
+				p->pos_base[i] = (int64_t)kSlideFirst + (p->pos_base[i] - (int64_t)kSlideFirst) % 32768;
+			if (level >= 5 && p->pos_base[i] + in_len[i] > 0xFFFFFFFFll) {
+				set_error("stream %d: %lld bytes behind position %lld do not fit one plan slot", i, (long long)in_len[i],
+				          (long long)p->pos_base[i]);
 				return B200Z_E_ARG;
 			}
 			if (hist->hist_mask && hist->hist_mask[i]) p->hist_mask[i].assign(hist->hist_mask[i], hist->hist_mask[i] + H);
@@ -1921,14 +2013,20 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 			uint32_t *rnd_symoff = ws.at(p->o_rnd_symoff);
 			if (p->n_chunks)
 				k_parse_chunk<<<p->n_chunks, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, ws.at(p->o_chunks), rnd_off,
-				                                                 recs, ents, hist, bias, lp, p->strategy, parse_warm());
+				                                                 recs, ents, hist, bias, ws.at(p->o_entry), lp, p->strategy, parse_warm(),
+				                                                 p->end_mode);
 			k_parse_fix<<<n, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, rnd_off, recs, ents, p->parse_chunk, hist,
-			                                      bias, lp, p->strategy);
+			                                      bias, lp, p->strategy, p->end_mode);
 			k_parse_scan<<<n, 256, 0, s>>>(d_in, in_off, in_len, rnd_off, recs, rnd_symoff, sym, nsyms, nblocks, blk_off, blk_start,
 			                               blk_ptop, hist, p->end_mode);
 			if (p->n_rgroups)
 				k_parse_gather<<<p->n_rgroups, 128, 0, s>>>(sym_local, sym, in_off, in_len, ws.at(p->o_rgroups), rnd_off, recs,
 				                                           rnd_symoff, blk_off, blk_start, blk_ptop, hist);
+			if (p->end_mode == B200Z_END_NONE) {
+				k_parse_cut<<<(n + 127) / 128, 128, 0, s>>>(d_in, link, mt, in_off, in_len, rnd_off, recs, rnd_symoff, nblocks, bias,
+				                                            ws.at(p->o_entry), ws.at(p->o_cut), n, lp, p->strategy);
+				p->cut_ready = true;
+			}
 		}
 		p->mark(s, "k_plan");
 		k_plan<<<p->n_blkmax, kPlanThreads, 0, s>>>(sym, in_off, in_len, nsyms, nblocks, blk_off, blk_desc, blk_start, blk_ptop,
@@ -1940,13 +2038,64 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 		k_emit<<<p->n_blkmax, 256, 0, s>>>(d_in, sym, d_out, in_off, out_off, nblocks, blk_off, blk_desc, meta, tables);
 	}
 	p->mark(s, "checksum");
-	if (p->wrap != B200Z_WRAP_RAW && d_check) {
+	// (an open run leaves the running checksum alone: its caller knows which of the bytes the run covered)
+	if (p->wrap != B200Z_WRAP_RAW && d_check && p->end_mode != B200Z_END_NONE) {
 		int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at(p->o_ck_off), ws.at(p->o_ck_len), n,
 		                         ws.at(p->o_ck_desc), p->n_ck_tiles, ws.at(p->o_ck_acc), d_check, p->check_seeded ? 0 : 1, s);
 		if (rc) return rc;
 	}
 	p->mark(s, "end");
 	B200Z_CUDA(cudaGetLastError());
+	return B200Z_OK;
+}
+
+int deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry) {
+	DeflatePlan *p = static_cast<DeflatePlan *>(plan);
+	if (p->level < 5) {
+		set_error("entry states are for levels 5-9");
+		return B200Z_E_UNSUPPORTED;
+	}
+	std::vector<RoundRec> v(p->entry);
+	for (int i = 0; i < p->n; i++) {
+		const b200z_parse_entry &e = entry[i];
+		const int64_t H = p->hist.empty() ? 0 : p->hist[i];
+		const int64_t data = p->in_len[i] - H;
+		const bool pending = e.match_len >= kMinMatch;
+		// with nothing pending matchLen is MIN_MATCH - 1; a byte left pending lies in the data, and so does its match
+		if (e.prev_available < 0 || e.prev_available > 1 || e.match_len < kMinMatch - 1 || e.match_len > kMaxMatch ||
+		    (pending && (!e.prev_available || e.match_dist < 1 || e.match_dist > kMaxDist || e.match_dist > H)) ||
+		    (!pending && e.match_dist != 0) || (e.prev_available && data < (pending ? e.match_len : 1))) {
+			set_error("stream %d: entry state (prev_available %d, match_len %d, match_dist %lld) with %lld history and %lld data bytes",
+			          i, e.prev_available, e.match_len, (long long)e.match_dist, (long long)H, (long long)data);
+			return B200Z_E_ARG;
+		}
+		v[i].p = (uint32_t)(H + e.prev_available);
+		v[i].mlen = (uint32_t)e.match_len;
+		v[i].mstart = pending ? (uint32_t)(H - e.match_dist) : 0u;
+		v[i].prevAvail = (uint32_t)e.prev_available;
+	}
+	const int rc = p->ws.write(p->o_entry, v);
+	if (rc == B200Z_OK) p->entry = v;
+	return rc;
+}
+
+int deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, cudaStream_t s) {
+	DeflatePlan *p = static_cast<DeflatePlan *>(plan);
+	if (p->end_mode != B200Z_END_NONE || !p->cut_ready) {
+		set_error("a cut is reported after a run of a B200Z_END_NONE plan");
+		return B200Z_E_STATE;
+	}
+	std::vector<RoundRec> v((size_t)p->n);
+	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->o_cut), sizeof(RoundRec) * v.size(), cudaMemcpyDeviceToHost, s));
+	B200Z_CUDA(cudaStreamSynchronize(s));
+	for (int i = 0; i < p->n; i++) {
+		const int64_t H = p->hist.empty() ? 0 : p->hist[i];
+		const int64_t pos = (int64_t)v[i].p - v[i].prevAvail; // the first byte not written
+		covered[i] = pos - H;
+		next[i].prev_available = (int32_t)v[i].prevAvail;
+		next[i].match_len = (int32_t)v[i].mlen;
+		next[i].match_dist = v[i].mlen >= (uint32_t)kMinMatch ? pos - (int64_t)v[i].mstart : 0;
+	}
 	return B200Z_OK;
 }
 

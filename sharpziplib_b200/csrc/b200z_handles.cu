@@ -78,6 +78,12 @@ static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const ui
 // =====================================================================================================
 // Streaming handles
 // =====================================================================================================
+// Levels 5-9 compress a long stream in open runs (B200Z_END_NONE) of this many new bytes, plus what the run in front left
+// behind its cut: a plan's workspace grows with its input (about 3.7 GB for 256 MiB), and the output flows while input
+// arrives.  A segment up to this size runs as one plan, as it always has.
+constexpr int64_t kOpenRunBytes = 256ll << 20;
+constexpr b200z_parse_entry kCleanEntry = {0, kMinMatch - 1, 0};
+
 struct DeflaterH {
 	int level = 6, strategy = 0;
 	bool raw = false;
@@ -92,6 +98,11 @@ struct DeflaterH {
 	bool dict_set = false, deflate_called = false, started = false;
 	uint32_t dict_adler = 0;
 	std::vector<uint8_t> input;    // everything SetInput handed over and not yet compressed
+	// levels 5-9: the parse state the next run starts from, the bytes at the front of `input` that the last open run saw
+	// but left behind its cut, and whether that run's output is still being handed out
+	b200z_parse_entry entry = kCleanEntry;
+	int64_t carried = 0;
+	bool draining = false;
 	std::vector<uint8_t> pending;  // produced bytes not yet drained by Deflate()
 	size_t pending_pos = 0;
 	HostBits tail;                 // sub-byte tail carried between device runs
@@ -119,9 +130,23 @@ static void deflater_remember(DeflaterH *d, const uint8_t *seg, size_t len, size
 	d->window_seen += (int64_t)len;
 }
 
-static int deflater_run_device(DeflaterH *d, int end_mode) {
-	// compresses d->input as the next segment of the stream; END_FLUSH keeps the stream open and may end inside a byte
-	const int64_t len = (int64_t)d->input.size();
+static void deflater_header(DeflaterH *d) {
+	if (!d->header_done && !d->raw) {
+		uint8_t hd[2];
+		zlib_header(d->level, hd, d->dict_set);
+		d->pending.push_back(hd[0]);
+		d->pending.push_back(hd[1]);
+		if (d->dict_set) { // DICTID = Adler-32 of the whole dictionary, MSB first (:455-461)
+			for (int sh = 24; sh >= 0; sh -= 8) d->pending.push_back((uint8_t)(d->dict_adler >> sh));
+		}
+	}
+	d->header_done = true;
+}
+
+static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
+	// compresses the first `len` bytes of d->input as the next segment of the stream; END_FLUSH keeps the stream open and may
+	// end inside a byte; END_NONE (levels 5-9) writes the blocks that closed and keeps the bytes behind them for the next run
+	const bool open = end_mode == B200Z_END_NONE;
 	const int64_t H = (int64_t)d->history.size();
 	const bool continuing = d->started; // an earlier segment (possibly empty) has been emitted
 	b200z_history hs;
@@ -156,20 +181,38 @@ static int deflater_run_device(DeflaterH *d, int end_mode) {
 	int rc = b200z_deflate_plan_create_ex(1, &len, d->level, d->strategy, d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB, end_mode,
 	                                      (hs.kind != B200Z_HIST_NONE || d->level <= 4) ? &hs : nullptr, &plan);
 	if (rc) return rc;
+	if (d->level >= 5) rc = b200z_deflate_plan_set_entry(plan, &d->entry);
 	std::vector<uint8_t> slot;
 	const uint8_t *inp = d->input.data();
 	if (H) {
 		slot.reserve((size_t)(H + len));
 		slot.insert(slot.end(), d->history.begin(), d->history.end());
-		slot.insert(slot.end(), d->input.begin(), d->input.end());
+		slot.insert(slot.end(), d->input.begin(), d->input.begin() + len);
 		inp = slot.data();
 	}
 	const uint32_t seed = d->adler; // a plan with history continues the running checksum (hs.check_seeded)
-	rc = handle_run(plan, d->st, inp, (hs.kind != B200Z_HIST_NONE && !d->raw) ? &seed : nullptr);
+	if (!rc) rc = handle_run(plan, d->st, inp, (hs.kind != B200Z_HIST_NONE && !d->raw && !open) ? &seed : nullptr);
 	const PipeMeta &r = d->st.h;
 	if (!rc && (r.status[0] & 0xFF) != B200Z_OK) {
 		rc = r.status[0] & 0xFF;
 		set_error("device deflate failed with status %d", rc);
+	}
+	int64_t covered = len; // bytes of input this run is done with
+	b200z_parse_entry next = kCleanEntry;
+	if (!rc && open) {
+		rc = b200z_deflate_plan_get_cut(plan, &covered, &next, nullptr);
+		if (!rc && covered <= 0) { // (a run of more than 16384 * 258 + 262 bytes always closes a block)
+			set_error("open run of %lld bytes closed no block", (long long)len);
+			rc = B200Z_E_INTERNAL;
+		}
+		if (!rc && !d->raw) {
+			// the Adler-32 goes on over the covered bytes, read from the copy of the input the run left on the device
+			const int64_t off = b200z_plan_data_offset(plan, 0);
+			cudaError_t e = cudaMemcpy(d->st.d.check, &d->adler, 4, cudaMemcpyHostToDevice);
+			if (e == cudaSuccess && !(rc = b200z_checksum_batch_device(1, d->st.din.p, &off, &covered, 1, d->st.d.check, nullptr)))
+				e = cudaMemcpy(&d->adler, d->st.d.check, 4, cudaMemcpyDeviceToHost);
+			if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpy (running Adler-32)", __FILE__, __LINE__);
+		}
 	}
 	if (!rc) {
 		const uint8_t *o = d->st.hout.p + plan->out_off[0];
@@ -182,17 +225,40 @@ static int deflater_run_device(DeflaterH *d, int end_mode) {
 		d->tail.count = (int)(bits & 7);
 		d->tail.bits = d->tail.count ? (seg[(size_t)whole] & ((1u << d->tail.count) - 1u)) : 0u;
 		if (end_mode == B200Z_END_FINISH) d->tail.align(d->pending); // FINISHING_STATE: AlignToByte (:507)
-		if (!d->raw) d->adler = r.check[0];
+		if (!d->raw && !open) d->adler = r.check[0];
 		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run)
-		d->total_in += d->level == 0 ? (int64_t)(uint32_t)(d->sstate.input_off - stored_before) : len;
+		d->total_in += d->level == 0 ? (int64_t)(uint32_t)(d->sstate.input_off - stored_before) : covered;
 		d->started = true;
-		deflater_remember(d, d->input.data(), (size_t)len, 2);
-		d->input.clear();
-		d->chunks.clear();
-		d->undrained = false;
+		// every position in front of a cut went through InsertString; a flush leaves the last two out
+		deflater_remember(d, d->input.data(), (size_t)covered, open ? 0 : 2);
+		d->input.erase(d->input.begin(), d->input.begin() + covered);
+		d->entry = next;
+		d->carried = len - covered;
+		if (!open) {
+			d->chunks.clear();
+			d->undrained = false;
+		}
 	}
 	b200z_plan_destroy(plan);
 	return rc;
+}
+
+// Levels 5-9: while more than one run's worth of input is buffered, the front of it is compressed in open runs and their
+// output is due at once.  Each run takes the bytes its predecessor left behind the cut plus at most kOpenRunBytes more,
+// so it is longer than a block can be and always ends in a cut: no run is repeated on the same bytes.
+static int deflater_open_runs(DeflaterH *d) {
+	while (d->level >= 5 && (int64_t)d->input.size() > kOpenRunBytes) {
+		if (d->pending_pos == d->pending.size()) {
+			d->pending.clear();
+			d->pending_pos = 0;
+		}
+		deflater_header(d);
+		const int64_t len = std::min<int64_t>((int64_t)d->input.size(), d->carried + kOpenRunBytes);
+		int rc = deflater_run_device(d, B200Z_END_NONE, len);
+		if (rc) return rc;
+		d->draining = true;
+	}
+	return B200Z_OK;
 }
 
 // ---- Inflater handle ----------------------------------------------------------------------------------
@@ -377,6 +443,9 @@ int b200z_deflater_reset(void *h) { // Deflater.Reset :204-210 keeps level and s
 	d->chunks.clear();
 	d->undrained = false;
 	d->sstate = b200z_stored_state{0, 0, 0, 0};
+	d->entry = kCleanEntry;
+	d->carried = 0;
+	d->draining = false;
 	return B200Z_OK;
 }
 int b200z_deflater_set_level(void *h, int level) {
@@ -448,8 +517,10 @@ int b200z_deflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 		return B200Z_E_ARG;
 	}
 	// one plan slot addresses 4 GiB - 64 KiB (32-bit positions, the window phase included): refuse what could not be
-	// compressed instead of accepting it and failing at Flush() / Finish()
-	if ((int64_t)d->input.size() + len + 32768 > 0xFFFF0000ll || d->window_seen + (int64_t)d->input.size() + len > 0xFFFF0000ll) {
+	// compressed instead of accepting it and failing at Flush() / Finish().  Levels 5-9 run long input in open runs, and
+	// their plans take a stream position of any size.
+	if (d->level <= 4 &&
+	    ((int64_t)d->input.size() + len + 32768 > 0xFFFF0000ll || d->window_seen + (int64_t)d->input.size() + len > 0xFFFF0000ll)) {
 		set_error("Deflater handle: more than 4 GiB - 64 KiB in one stream (TotalIn %lld, %lld buffered, %d more): use several "
 		          "streams or the batch API",
 		          (long long)d->total_in, (long long)d->input.size(), len);
@@ -484,20 +555,15 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 	*produced = 0;
 	d->deflate_called = true;
 	if (!d->flushing && !d->finishing) d->undrained = false; // BUSY_STATE: the engine takes everything SetInput handed over
+	if (!d->finished) { // (also in front of a Flush() / Finish() run: no run sees more than one run's worth of new input)
+		int rc = deflater_open_runs(d);
+		if (rc) return rc;
+	}
 	// make output due (Deflater.Deflate :427-522)
 	if (!d->finished && d->pending_pos == d->pending.size() && (d->flushing || d->finishing)) {
 		d->pending.clear();
 		d->pending_pos = 0;
-		if (!d->header_done && !d->raw) {
-			uint8_t hd[2];
-			zlib_header(d->level, hd, d->dict_set);
-			d->pending.push_back(hd[0]);
-			d->pending.push_back(hd[1]);
-			if (d->dict_set) { // DICTID = Adler-32 of the whole dictionary, MSB first (:455-461)
-				for (int sh = 24; sh >= 0; sh -= 8) d->pending.push_back((uint8_t)(d->dict_adler >> sh));
-			}
-		}
-		d->header_done = true;
+		deflater_header(d);
 		if (d->finishing) {
 			if (d->flushed_once) {
 				// Flush() already emitted every block + the sync padding; Finish adds the final empty block:
@@ -511,7 +577,7 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 					d->tail.align(d->pending);
 				}
 			} else {
-				int rc = deflater_run_device(d, B200Z_END_FINISH);
+				int rc = deflater_run_device(d, B200Z_END_FINISH, (int64_t)d->input.size());
 				if (rc) return rc;
 			}
 			if (!d->raw) {
@@ -523,7 +589,7 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 			d->finished = true;
 		} else {
 			// sync flush (level 0 skips the padding, :488)
-			int rc = deflater_run_device(d, B200Z_END_FLUSH);
+			int rc = deflater_run_device(d, B200Z_END_FLUSH, (int64_t)d->input.size());
 			if (rc) return rc;
 			d->flushed_once = true;
 			d->flushing = false;
@@ -535,14 +601,17 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 	d->pending_pos += take;
 	d->total_out += (int64_t)take;
 	*produced = (int32_t)take;
+	if (d->pending_pos == d->pending.size()) d->draining = false;
 	return B200Z_OK;
 }
 int b200z_deflater_needs_input(void *h, int *flag) {
 	// DeflaterEngine.NeedsInput (:187-190): false between SetInput and the Deflate() call that takes the bytes.  The
 	// handle copies on SetInput, but it reports what the reference reports: DeflaterOutputStream.Write calls Deflate()
 	// exactly while this is false (Streams/DeflaterOutputStream.cs:245-275), and whether that call happened before
-	// Flush() / Finish() changes the bytes at levels 0-4 (b200z_history.undrained_last)
-	*flag = ((DeflaterH *)h)->undrained ? 0 : 1;
+	// Flush() / Finish() changes the bytes at levels 0-4 (b200z_history.undrained_last).  The output of an open run also
+	// keeps it false until it has been handed out, as the reference's engine holds input while its output is pending.
+	const DeflaterH *d = (const DeflaterH *)h;
+	*flag = (d->undrained || d->draining) ? 0 : 1;
 	return B200Z_OK;
 }
 int b200z_deflater_is_finished(void *h, int *flag) {

@@ -260,6 +260,10 @@ int b200z_deflate_pipeline_create(int32_t n, const int64_t *in_len, int level, i
 		return B200Z_E_ARG;
 	}
 	if (level == -1) level = 6;
+	if (end_mode == B200Z_END_NONE) {
+		set_error("pipelines and batch calls return whole streams: open runs (B200Z_END_NONE) need the deflate plan calls");
+		return B200Z_E_UNSUPPORTED;
+	}
 	b200z_plan *plan = nullptr;
 	// gzip: the plan delivers the raw stream and the CRC-32; collect() writes header and trailer (GzipOutputStream.cs:315-375)
 	int rc = b200z_deflate_plan_create(n, in_len, level, strategy, wrap == B200Z_WRAP_GZIP ? B200Z_WRAP_RAW_CRC32 : wrap, end_mode, &plan);
