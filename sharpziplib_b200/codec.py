@@ -7,6 +7,16 @@ import numpy as np
 from . import _lib
 from .checksum import _as_u8
 
+INT32_MAX = 0x7FFFFFFF  # SetInput's count is a C# int, and an int32_t in the C-ABI
+
+
+def _input(data, offset, count):
+    """the span SetInput hands to the library; a longer one is refused rather than cut to its count's low 32 bits"""
+    a = _as_u8(data, offset, count)
+    if a.size > INT32_MAX:
+        raise ValueError("count: %d bytes in one SetInput (at most %d)" % (a.size, INT32_MAX))
+    return a
+
 
 class DeflateStrategy:
     """Zip/Compression/DeflaterEngine.cs:9-28"""
@@ -54,7 +64,7 @@ class Deflater:
         _lib.raise_for(_lib.lib().b200z_deflater_set_dictionary(self._h, a.ctypes.data, a.size))
 
     def SetInput(self, input, offset=0, count=None):  # :308/:331
-        a = _as_u8(input, offset, count)
+        a = _input(input, offset, count)
         _lib.raise_for(_lib.lib().b200z_deflater_set_input(self._h, a.ctypes.data if a.size else None, a.size))
 
     def Flush(self):  # :252
@@ -130,7 +140,7 @@ class Inflater:
         _lib.raise_for(_lib.lib().b200z_inflater_set_dictionary(self._h, a.ctypes.data, a.size))
 
     def SetInput(self, buffer, index=0, count=None):  # :629/:653
-        a = _as_u8(buffer, index, count)
+        a = _input(buffer, index, count)
         _lib.raise_for(_lib.lib().b200z_inflater_set_input(self._h, a.ctypes.data if a.size else None, a.size))
 
     def Inflate(self, buffer, offset=0, count=None):

@@ -153,7 +153,7 @@ static int checksum_host(int kind, const uint8_t *buf, int64_t len, uint32_t *va
 	B200Z_CUDA(cudaMemcpy(d_len, &len, 8, cudaMemcpyHostToDevice));
 	B200Z_CUDA(cudaMemcpy(d_val, value, 4, cudaMemcpyHostToDevice));
 	B200Z_CUDA(cudaMemcpy(d_tiles, tiles.data(), tb, cudaMemcpyHostToDevice));
-	rc = checksum_launch(kind, d.p, d_off, d_len, 1, d_tiles, (int32_t)tiles.size(), d_acc, d_val, 0, 0);
+	rc = checksum_launch(kind, d.p, d_off, d_len, 1, d_tiles, (int32_t)tiles.size(), d_acc, d_val, 0, 0, false);
 	if (rc) return rc;
 	B200Z_CUDA(cudaMemcpy(value, d_val, 4, cudaMemcpyDeviceToHost));
 	return B200Z_OK;
@@ -473,7 +473,7 @@ int b200z_checksum_batch_device(int kind, const uint8_t *d_data, const int64_t *
 	B200Z_CUDA(cudaMemcpyAsync(d_off, off, 8ull * n, cudaMemcpyHostToDevice, s));
 	B200Z_CUDA(cudaMemcpyAsync(d_len, len, 8ull * n, cudaMemcpyHostToDevice, s));
 	if (tb) B200Z_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tb, cudaMemcpyHostToDevice, s));
-	rc = checksum_launch(kind, d_data, d_off, d_len, n, d_tiles, (int32_t)tiles.size(), d_acc, d_value, 0, s);
+	rc = checksum_launch(kind, d_data, d_off, d_len, n, d_tiles, (int32_t)tiles.size(), d_acc, d_value, 0, s, false);
 	B200Z_CUDA(cudaStreamSynchronize(s)); // the pageable descriptor copies above must finish before `tiles` dies
 	B200Z_CUDA(cudaFreeAsync(meta, s));
 	return rc;

@@ -43,7 +43,7 @@ int checksum_tiles(const int64_t *len, int32_t n, std::vector<CkTile> &tiles, in
 	for (int32_t i = 0; i < n; i++) {
 		const int64_t L = len[i];
 		const size_t first = tiles.size();
-		for (int64_t s = 0; s < L; s += kCkTile) tiles.push_back(CkTile{i, (uint32_t)s, 0u, dynamic ? kCkDynamic : 0u});
+		for (int64_t s = 0; s < L; s += kCkTile) tiles.push_back(CkTile{(uint64_t)s, i, 0u});
 		if (dynamic) continue; // len[] are capacities: the kernel works the multipliers out from the device-side lengths
 		// multipliers from the last tile backwards: one mulmod per tile
 		uint32_t m = 1u << 31; // x^0
@@ -67,18 +67,18 @@ __global__ void k_ck_zero(uint64_t *acc, int n2) {
 template <int KIND>
 __global__ void __launch_bounds__(kCkThreads)
     k_checksum(const uint8_t *__restrict__ data, const int64_t *__restrict__ off, const int64_t *__restrict__ len,
-               const CkTile *__restrict__ tiles, unsigned long long *__restrict__ acc) {
+               const CkTile *__restrict__ tiles, int dynamic, unsigned long long *__restrict__ acc) {
 	__shared__ uint32_t s_words[kCkThreads * 33];
 	__shared__ uint32_t s_tab[4][256];
 	__shared__ unsigned long long s_red[2][kCkThreads / 32];
 	CkTile td = tiles[blockIdx.x];
 	const uint64_t n = (uint64_t)len[td.stream];
-	if ((uint64_t)td.start >= n) return; // tiles laid out for a capacity (inflate output): nothing of this stream here
+	if (td.start >= n) return; // tiles laid out for a capacity (inflate output): nothing of this stream here
 	const uint8_t *src = data + off[td.stream] + td.start;
 	const uint32_t tlen = n - td.start < (uint64_t)kCkTile ? (uint32_t)(n - td.start) : (uint32_t)kCkTile;
-	if (td.pad == kCkDynamic) {
+	if (dynamic) {
 		// the length was not known when the tiles were made: derive the multiplier from the bytes behind this tile
-		const uint64_t after = n - ((uint64_t)td.start + tlen);
+		const uint64_t after = n - (td.start + tlen);
 		td.mult = KIND == 0 ? crc_xpow8(after) : (uint32_t)(after % kAdlerBase);
 	}
 	const int tid = threadIdx.x;
@@ -201,14 +201,14 @@ __global__ void k_ck_final(const int64_t *__restrict__ len, int n, const unsigne
 // acc: 2 x uint64 per stream of scratch
 int checksum_launch(int kind, const uint8_t *d_data, const int64_t *d_off, const int64_t *d_len, int32_t n,
                     const CkTile *d_tiles, int32_t n_tiles, unsigned long long *d_acc, uint32_t *d_value, int fresh,
-                    cudaStream_t s) {
+                    cudaStream_t s, bool dynamic) {
 	int rc = checksum_init_tables();
 	if (rc) return rc;
 	if (n == 0) return B200Z_OK;
 	k_ck_zero<<<(2 * n + 255) / 256, 256, 0, s>>>(reinterpret_cast<uint64_t *>(d_acc), 2 * n);
 	if (n_tiles) {
-		if (kind == 0) k_checksum<0><<<n_tiles, kCkThreads, 0, s>>>(d_data, d_off, d_len, d_tiles, d_acc);
-		else k_checksum<1><<<n_tiles, kCkThreads, 0, s>>>(d_data, d_off, d_len, d_tiles, d_acc);
+		if (kind == 0) k_checksum<0><<<n_tiles, kCkThreads, 0, s>>>(d_data, d_off, d_len, d_tiles, dynamic ? 1 : 0, d_acc);
+		else k_checksum<1><<<n_tiles, kCkThreads, 0, s>>>(d_data, d_off, d_len, d_tiles, dynamic ? 1 : 0, d_acc);
 	}
 	if (kind == 0) k_ck_final<0><<<(n + 127) / 128, 128, 0, s>>>(d_len, n, d_acc, d_value, fresh);
 	else k_ck_final<1><<<(n + 127) / 128, 128, 0, s>>>(d_len, n, d_acc, d_value, fresh);

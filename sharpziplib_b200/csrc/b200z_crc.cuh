@@ -53,12 +53,11 @@ B200Z_HD uint32_t crc_table0_entry(uint32_t i) {
 	return res;
 }
 
-constexpr uint32_t kCkDynamic = 0xD1CEu; // CkTile.pad: multiplier to be computed on the device (length known only there)
 struct CkTile {
+	uint64_t start; // first byte of the tile inside its stream (64-bit: a stream may be longer than 4 GiB)
 	int32_t stream;
-	uint32_t start; // first byte of the tile inside its stream
 	uint32_t mult;  // CRC: x^(8 * bytes after this tile) ; Adler: bytes after this tile mod 65521
-	uint32_t pad;
 };
+static_assert(sizeof(CkTile) == 16, "one tile descriptor per 16 bytes");
 
 } // namespace b200z

@@ -2041,7 +2041,7 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 	// (an open run leaves the running checksum alone: its caller knows which of the bytes the run covered)
 	if (p->wrap != B200Z_WRAP_RAW && d_check && p->end_mode != B200Z_END_NONE) {
 		int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at(p->o_ck_off), ws.at(p->o_ck_len), n,
-		                         ws.at(p->o_ck_desc), p->n_ck_tiles, ws.at(p->o_ck_acc), d_check, p->check_seeded ? 0 : 1, s);
+		                         ws.at(p->o_ck_desc), p->n_ck_tiles, ws.at(p->o_ck_acc), d_check, p->check_seeded ? 0 : 1, s, false);
 		if (rc) return rc;
 	}
 	p->mark(s, "end");

@@ -1199,7 +1199,7 @@ int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 	if (wrap != B200Z_WRAP_RAW) {
 		p->mark(s, "checksum");
 		int rc = checksum_launch(wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_out, out_off, d_out_len, n, ws.at(p->o_ck_desc), p->n_ck_tiles,
-		                         ws.at(p->o_ck_acc), d_check, 1, s);
+		                         ws.at(p->o_ck_acc), d_check, 1, s, true);
 		if (rc) return rc;
 		if (framed) k_wrap_tail<<<(n + 127) / 128, 128, 0, s>>>(d_in, in_off, in_len, n, wrap, d_in_used, d_out_len, d_check, d_status);
 	}

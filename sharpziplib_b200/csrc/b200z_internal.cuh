@@ -210,9 +210,11 @@ int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t
                      uint32_t *d_check, int64_t *d_in_used, cudaStream_t s);
 // checksum over n device buffers (kind 0 = CRC32, 1 = Adler32); d_acc = 2 x uint64 scratch per stream;
 // value in/out (device uint32), `fresh` != 0 starts from the Reset() value instead of reading d_value.
+// `dynamic`: the tiles were laid over capacities (checksum_tiles(..., dynamic = true)) and d_len holds the real lengths,
+// known only on the device: the kernel skips the tiles past them and works the multipliers out itself.
 int checksum_launch(int kind, const uint8_t *d_data, const int64_t *d_off, const int64_t *d_len, int32_t n,
                     const CkTile *d_tiles, int32_t n_tiles, unsigned long long *d_acc, uint32_t *d_value, int fresh,
-                    cudaStream_t s);
+                    cudaStream_t s, bool dynamic);
 int checksum_tiles(const int64_t *len, int32_t n, std::vector<CkTile> &tiles, int kind, bool dynamic = false);
 int checksum_init_tables();
 } // namespace b200z

@@ -5,8 +5,8 @@ import io
 import struct
 
 from ._lib import SharpZipBaseException
-from .checksum import Crc32
-from .codec import Deflater, Inflater
+from .checksum import Crc32, _as_u8
+from .codec import INT32_MAX, Deflater, Inflater
 
 
 class DeflaterOutputStream:
@@ -45,8 +45,12 @@ class DeflaterOutputStream:
             raise SharpZipBaseException("DeflaterOutputStream can't deflate all input?")
 
     def Write(self, buffer, offset=0, count=None):  # :506-510
-        self.deflater_.SetInput(buffer, offset, count)
-        self._deflate(False)
+        a = _as_u8(buffer, offset, count)
+        # a C# caller cannot pass more than int.MaxValue bytes at once: a longer span goes as consecutive Writes of 1 GiB
+        step = max(a.size, 1) if a.size <= INT32_MAX else 1 << 30
+        for p in range(0, max(a.size, 1), step):
+            self.deflater_.SetInput(a[p:p + step])
+            self._deflate(False)
 
     def WriteByte(self, value):  # Stream.WriteByte -> Write of one byte (:495-504)
         self.Write(bytes([value & 0xFF]))
