@@ -36,7 +36,7 @@ enum {
 	B200Z_END_FINISH = 0,       /* SetInput* -> Finish()                       (Deflater.cs:262; DeflaterOutputStream.Finish :100) */
 	B200Z_END_FLUSH_FINISH = 1, /* SetInput* -> Flush() -> Finish()            (test pattern InflaterDeflaterTests.cs:49-62)      */
 	B200Z_END_FLUSH = 2,        /* SetInput* -> Flush(), stream continues      (Deflater.cs:252, sync padding :486-504)           */
-	B200Z_END_NONE = 3          /* SetInput* -> Deflate(), stream continues: levels 5-9 plans only, see "open runs" below       */
+	B200Z_END_NONE = 3          /* SetInput* -> Deflate(), stream continues: plans only, see "open runs" below                 */
 };
 
 const char *b200z_last_error(void);
@@ -92,7 +92,9 @@ typedef struct b200z_plan b200z_plan;
  * called, DeflateFast at > 65274; DeflateStored cuts blocks by what it has seen so far): chunk_count / chunk_len give the
  * SetInput calls that delivered a stream's data, each followed by Deflate() until IsNeedingInput as DeflaterOutputStream
  * .Write does (Streams/DeflaterOutputStream.cs:506-510); without them one SetInput with everything is assumed.  Levels 5-9
- * ignore the schedule (their output does not depend on it).
+ * ignore the schedule (their output does not depend on it).  At levels 0-4 the positions of a continued stream live in the
+ * engine state: a plan reduces its slides / input_off by the same multiple of 32768 (the window phase stays), so a stream
+ * may go on past 4 GiB, and pos_base may have any size.
  * Input slot i of such a plan holds hist_len[i] history bytes directly followed by the in_len[i] data bytes;
  * b200z_plan_in_offset(i) is the start of the history.  The checksum covers the data only; with check_seeded the
  * d_check array handed to b200z_plan_run carries the running values in and the updated values out (Adler32.Update /
@@ -128,8 +130,9 @@ typedef struct b200z_stored_state { /* DeflateStored's fields between Deflate() 
 } b200z_stored_state;
 int64_t b200z_engine_state_bytes(void);
 
-/* ---- open runs (levels 5-9) -----------------------------------------------------------------------------------
- * A stream compressed in pieces without Flush(): what Deflate() leaves behind in BUSY_STATE.  Without a flush the
+/* ---- open runs ---------------------------------------------------------------------------------------------------
+ * A stream compressed in pieces without Flush(): what Deflate() leaves behind in BUSY_STATE.
+ * Levels 5-9: without a flush the
  * reference's output at levels 5-9 does not depend on how the input arrived (trap T9); blocks end only by the
  * 16384-symbol rule, and at the end of a block DeflateSlow carries nothing but its parse state.  A B200Z_END_NONE run
  * parses the loop tops with at least MIN_LOOKAHEAD (262) bytes ahead, writes only the blocks the symbol rule closed
@@ -140,7 +143,15 @@ int64_t b200z_engine_state_bytes(void);
  * the bytes of one run over everything.
  * The entry state (default: a clean start): with prev_available, data byte 0 is the byte the previous run left
  * pending (trap T10) and the parse goes on at byte 1 with match_len / match_dist, a match found at byte 0 (distance
- * back from byte 0; only read when match_len >= 3).  Without it match_len is 2. */
+ * back from byte 0; only read when match_len >= 3).  Without it match_len is 2.
+ * Levels 0-4: the run takes the BUSY_STATE loops of its SetInput calls (chunk_len; undrained_last is ignored) and writes
+ * the blocks the engine itself closed (DeflateFast's 16384-symbol rule; DeflateStored's MAX_BLOCK_SIZE / MAX_DIST rule).
+ * Right behind such a block the engine holds no symbols, so the plan needs the engine state to write the cut into:
+ * engine_state (levels 1-4, overwritten on the device) or stored_state (level 0, overwritten when the plan is created);
+ * without it B200Z_E_UNSUPPORTED.  `covered` is the stream offset of blockStart there.  The bytes between it and the
+ * state's input_off are already in the window, and they are the first bytes of the next run's data.  That run continues
+ * (B200Z_HIST_CONTINUE) with at least 32768 bytes of history in front of `covered` (all there is near the start) and the
+ * schedule from get_cut_call.  Chaining runs this way gives exactly the bytes of one run over everything. */
 typedef struct b200z_parse_entry {
 	int32_t prev_available; /* 0 or 1 */
 	int32_t match_len;      /* 2, or 3..258 when a match is pending */
@@ -148,8 +159,14 @@ typedef struct b200z_parse_entry {
 } b200z_parse_entry;
 /* entry[n]: host array; valid for every end mode of a level 5-9 plan, read by every later run */
 int b200z_deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry);
-/* after a B200Z_END_NONE run: covered[n] and next[n] (host arrays); synchronises `cuda_stream` */
+/* after a B200Z_END_NONE run: covered[n] and next[n] (host arrays; next may be NULL at levels 0-4, where it is always the
+ * clean entry); synchronises `cuda_stream`.  covered[i] == 0: the run closed no block */
 int b200z_deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, void *cuda_stream);
+/* levels 0-4, after a B200Z_END_NONE run: call[n] (host array), per stream the index into its chunk_len (0 without a
+ * schedule) of the SetInput call in whose Deflate() loop the last written block closed.  The next run's schedule is the
+ * rest of that call measured from `covered` (its end minus covered, which may be 0), then the calls behind it: a run that
+ * starts inside a call does not begin a new one.  Synchronises `cuda_stream`. */
+int b200z_deflate_plan_get_cut_call(b200z_plan *plan, int32_t *call, void *cuda_stream);
 
 int b200z_deflate_plan_create_ex(int32_t n, const int64_t *in_len, int level, int strategy, int wrap, int end_mode,
                                  const b200z_history *hist, b200z_plan **plan);

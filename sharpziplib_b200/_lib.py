@@ -81,6 +81,7 @@ _SIGS = {
     "b200z_plan_data_offset": (C.c_int64, [C.c_void_p, C.c_int32]),
     "b200z_deflate_plan_set_entry": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200z_deflate_plan_get_cut": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_deflate_plan_get_cut_call": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_plan_destroy": (C.c_int, [C.c_void_p]),
     "b200z_plan_in_bytes": (C.c_int64, [C.c_void_p]),
     "b200z_plan_out_bytes": (C.c_int64, [C.c_void_p]),

@@ -70,7 +70,7 @@ class DeflatePlan(_Plan):
     """n independent streams, each what `new Deflater(level, true)` + SetInput(all) + Finish() would produce."""
 
     def __init__(self, in_lens, level=6, strategy=0, wrap=_lib.WRAP_RAW, end_mode=_lib.END_FINISH, dict_lens=None,
-                 chunk_lens=None, history=None, entry=None):
+                 chunk_lens=None, history=None, entry=None, state=None, undrained=None):
         """dict_lens: per-stream preset-dictionary bytes (Deflater.SetDictionary; at most 32506, the reference keeps the
         dictionary's tail) stored in the input slot directly in front of the stream's data.
         chunk_lens: per stream, the sizes of the SetInput calls that deliver its data (each followed by Deflate() until
@@ -79,11 +79,18 @@ class DeflatePlan(_Plan):
         (B200Z_HIST_CONTINUE); pos_bases are the data's stream offsets, of any size, bit_bases the bits (0..7) the previous
         run left in its last byte, masks per stream the history positions that are not in the hash chains (default: none,
         which is what a cut leaves).
-        end_mode=END_NONE (levels 5-9): an open run, see cut().
-        entry: per stream (prev_available, match_len, match_dist), the parse state to start from (set_entry)."""
+        end_mode=END_NONE: an open run, see cut().
+        entry: per stream (prev_available, match_len, match_dist), the parse state to start from (set_entry).
+        state (levels 0-4): the engine state carried between the runs of a stream -- at levels 1-4 n CUDA uint8 tensors of
+        engine_state_bytes() each (head[], prev[], DeflateFast's scalars, written by the run), at level 0 a uint8 array of
+        16 * n bytes (b200z_stored_state[n], overwritten when the plan is made).  With history the stream goes on from it;
+        history and chunk_lens may then come together.  undrained: per stream, Flush() / Finish() follows the last SetInput
+        without a Deflate() call in between."""
         lens = np.ascontiguousarray(in_lens, dtype=np.int64)
         h = C.c_void_p()
-        if history is not None:
+        if state is not None:
+            self._fast_state(lens, level, strategy, wrap, end_mode, dict_lens, chunk_lens, history, state, undrained, h)
+        elif history is not None:
             hl = np.ascontiguousarray(history[0], dtype=np.int64)
             pb = np.ascontiguousarray(history[1], dtype=np.int64)
             bb = np.ascontiguousarray(history[2], dtype=np.int32)
@@ -118,9 +125,39 @@ class DeflatePlan(_Plan):
                                                                   C.addressof(hs), C.byref(h)))
             self.dict_lens = dl
         self.in_lens = lens
+        self.level = level
         super().__init__(h, lens.size)
         if entry is not None:
             self.set_entry(entry)
+
+    def _fast_state(self, lens, level, strategy, wrap, end_mode, dict_lens, chunk_lens, history, state, undrained, h):
+        n = lens.size
+        if history is not None:
+            kind, hl = _lib.HIST_CONTINUE, np.ascontiguousarray(history[0], dtype=np.int64)
+            pb = np.ascontiguousarray(history[1], dtype=np.int64)
+            bb = np.ascontiguousarray(history[2], dtype=np.int32)
+        else:
+            kind = _lib.HIST_NONE if dict_lens is None else _lib.HIST_DICTIONARY
+            hl = np.zeros(n, np.int64) if dict_lens is None else np.ascontiguousarray(dict_lens, dtype=np.int64)
+            pb = bb = None
+        cl = chunk_lens if chunk_lens is not None else [[int(x)] for x in lens]
+        arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in cl]
+        counts = np.array([a.size for a in arrs], dtype=np.int32)
+        ptrs = (C.c_void_p * n)(*[a.ctypes.data if a.size else None for a in arrs])
+        und = np.ascontiguousarray(undrained if undrained is not None else np.zeros(n), dtype=np.int32)
+        if level == 0:
+            assert isinstance(state, np.ndarray) and state.dtype == np.uint8 and state.size == 16 * n
+            eng, st = None, state.ctypes.data
+        else:
+            assert len(state) == n
+            eng, st = (C.c_void_p * n)(*[t.data_ptr() for t in state]), None
+        hs = _lib.History(kind, 0, hl.ctypes.data, None if pb is None else pb.ctypes.data, None if bb is None else bb.ctypes.data,
+                          None, counts.ctypes.data, C.addressof(ptrs), und.ctypes.data,
+                          None if eng is None else C.addressof(eng), st)
+        _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(n, lens.ctypes.data, level, strategy, wrap, end_mode,
+                                                              C.addressof(hs), C.byref(h)))
+        self.dict_lens = hl
+        self._state = state  # (levels 1-4: the runs write it)
 
     def set_entry(self, entry):
         """per stream (prev_available, match_len, match_dist): the parse state the next runs start from"""
@@ -130,11 +167,18 @@ class DeflatePlan(_Plan):
 
     def cut(self, stream=None):
         """After an END_NONE run: (covered, entries) -- per stream the data bytes in front of the first block not written
-        (the next run's data starts there) and the (prev_available, match_len, match_dist) to enter that run with.
+        (the next run's data starts there) and the (prev_available, match_len, match_dist) to enter that run with.  At
+        levels 0-4 (covered, calls): the state is in the plan's `state`, and calls[i] is the SetInput call of chunk_lens[i]
+        the cut fell into -- the next run's calls are the rest of it from `covered` on, then the ones behind it.
         Synchronises the stream."""
         import torch
         s = stream if stream is not None else torch.cuda.current_stream()
         covered = np.zeros(self.n, dtype=np.int64)
+        if self.level <= 4:
+            calls = np.zeros(max(self.n, 1), dtype=np.int32)
+            _lib.raise_for(_lib.lib().b200z_deflate_plan_get_cut(self._h, covered.ctypes.data, None, s.cuda_stream))
+            _lib.raise_for(_lib.lib().b200z_deflate_plan_get_cut_call(self._h, calls.ctypes.data, s.cuda_stream))
+            return covered, [int(c) for c in calls[:self.n]]
         arr = (_lib.ParseEntry * max(self.n, 1))()
         _lib.raise_for(_lib.lib().b200z_deflate_plan_get_cut(self._h, covered.ctypes.data, arr, s.cuda_stream))
         return covered, [(e.prev_available, e.match_len, e.match_dist) for e in arr[:self.n]]

@@ -298,11 +298,20 @@ int b200z_deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entr
 
 int b200z_deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, void *cuda_stream) {
 	DeviceGuard guard(plan ? plan->device : -1);
-	if (!plan || plan->kind != 0 || (plan->n > 0 && (!covered || !next))) {
+	if (!plan || plan->kind != 0 || (plan->n > 0 && (!covered || (!next && plan->level >= 5)))) {
 		set_error("bad arguments");
 		return B200Z_E_ARG;
 	}
 	return deflate_plan_get_cut(plan, covered, next, (cudaStream_t)cuda_stream);
+}
+
+int b200z_deflate_plan_get_cut_call(b200z_plan *plan, int32_t *call, void *cuda_stream) {
+	DeviceGuard guard(plan ? plan->device : -1);
+	if (!plan || plan->kind != 0 || (plan->n > 0 && !call)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	return deflate_plan_get_cut_call(plan, call, (cudaStream_t)cuda_stream);
 }
 
 int b200z_inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, b200z_plan **plan) {

@@ -331,6 +331,18 @@ struct FastCarry {
 };
 constexpr int kFastStateBytes = 2 * 65536 + 64; // head[32768], prev[32768], FastCarry
 
+// inputOff and 32768 * slides only matter relative to each other and to the window (strstart and blockStart are window
+// indices, the phase of SlideWindow): a run entered with carried state drops the same multiple of 32768 from both, so that
+// no 32-bit field holds a stream-absolute position and a stream may go on past 4 GiB.  Returns the multiple dropped.
+B200Z_HD uint32_t carry_rebase(uint32_t &slides, uint32_t &inputOff) {
+	const uint32_t m = slides > 1u ? slides - 1u : 0u;
+	slides -= m;
+	inputOff -= 32768u * m;
+	return m;
+}
+// stream position (dictionary included, reduced like inputOff) of window index w
+B200Z_HD uint32_t fe_stream_pos(uint32_t slides, int w) { return 32768u * slides - 1u + (uint32_t)w; }
+
 B200Z_HD uint32_t fe_win(const FastEngine &e, int w) { return (uint32_t)e.in[(uint32_t)w + e.woff]; }
 
 B200Z_HD void fe_init(FastEngine &e, const uint8_t *in, uint32_t n, uint16_t *head, uint16_t *prev) {
@@ -375,8 +387,11 @@ B200Z_HD void fe_load(FastEngine &e, const FastCarry &c, const uint8_t *slot, ui
 	e.ins_h = c.ins_h;
 	e.slides = c.slides;
 	e.inputOff = c.inputOff;
-	e.n = c.inputOff; // nothing new is visible before the first SetInput of the segment
-	e.woff = 32768u * c.slides - 1u - (c.inputOff - hist); // slot byte 0 is stream byte inputOff - hist
+	carry_rebase(e.slides, e.inputOff);
+	e.n = e.inputOff; // nothing new is visible before the first SetInput of the segment
+	// slot byte `hist` is window index blockStart: the first byte no block has taken yet (behind a Flush() also strstart;
+	// behind the cut of an open run the bytes from there to inputOff are already in the window as lookahead)
+	e.woff = (uint32_t)hist - (uint32_t)c.blockStart;
 	e.nsym = 0;
 	e.coop = 0;
 }
@@ -561,33 +576,53 @@ B200Z_HDN int fe_deflate_fast(FastEngine &e, bool flush, bool finish, const Leve
 // One segment of a stream (everything up to a Flush() or Finish()), call pattern above.  The segment's bytes arrive in
 // `nchunks` SetInput calls, cum[i] bytes after the first i + 1 of them (nchunks == 0: one call with everything); each is
 // followed by Deflate() until IsNeedingInput.  For DeflateFast the result depends on that schedule (trap T9: FillWindow
-// slides at strstart >= 65274 when it is called, DeflateFast at > 65274), so the handle records it.
-// end_mode: B200Z_END_* (0 finish, 1 flush then finish, 2 flush).
-template <class EmitFn, class BlockFn>
-B200Z_HDN void fe_run(FastEngine &e, const LevelParams &lp, int strategy, int end_mode, EmitFn emit, BlockFn block,
-                      const uint32_t *cum = nullptr, int nchunks = 0, bool busy_last = true) {
-	const uint32_t seg_base = e.inputOff;
-	// slot byte 0 is stream byte 32768 * slides - 1 - woff; the segment is what the slot holds behind inputOff
-	const uint32_t seg_len = 32768u * e.slides - 1u - e.woff + e.slot_len - e.inputOff;
+// slides at strstart >= 65274 when it is called, DeflateFast at > 65274), so the handle records it.  The segment's data
+// starts at blockStart (the first byte no block has taken; after a cut some of it may already sit in the window).
+// end_mode: B200Z_END_* (0 finish, 1 flush then finish, 2 flush, 3 none).
+// End mode 3 is an open run: only the BUSY_STATE loops run, over every call of the schedule (busy_last is ignored), and
+// blocks end only by the 16384-symbol rule.  Right behind every block that closes, DeflateFast returns and the engine
+// carries nothing but its window, tables and scalars (strstart == blockStart, no symbol pending): cut(ci) is called there
+// with the index of the call in whose Deflate() loop the block closed.  The last cut is where the next run starts: its
+// schedule is the rest of call ci, from blockStart on, followed by the later calls.
+template <class EmitFn, class BlockFn, class CutFn>
+B200Z_HDN void fe_run(FastEngine &e, const LevelParams &lp, int strategy, int end_mode, EmitFn emit, BlockFn block, CutFn cut,
+                      const uint32_t *cum, int nchunks, bool busy_last) {
+	const bool open = end_mode == 3;
+	const uint32_t seg_base = fe_stream_pos(e.slides, e.blockStart);
+	const uint32_t seg_end = 32768u * e.slides - 1u - e.woff + e.slot_len; // stream position behind the slot
 	// busy_last = false: Flush() / Finish() follows the last SetInput directly, without a Deflate() call in between
 	const int nc = nchunks > 0 ? nchunks : 1;
+	bool closed = false;
+	auto blk = [&](uint32_t start, bool ok, bool last) {
+		block(start, ok, last);
+		closed = true;
+	};
 	for (int ci = 0; ci < nc; ci++) {
-		e.n = seg_base + (nchunks > 0 ? cum[ci] : seg_len);
-		if (ci == nc - 1 && !busy_last) break;
+		e.n = nchunks > 0 ? seg_base + cum[ci] : seg_end;
+		if (ci == nc - 1 && !busy_last && !open) break;
 		// BUSY_STATE: Deflater.Deflate -> engine.Deflate(false, false) until it reports "needs input" (:104-137)
 		for (;;) {
 			fe_fill_window(e);
-			if (fe_deflate_fast(e, false, false, lp, strategy, emit, block) == kFeFalse) break;
+			closed = false;
+			const int r = fe_deflate_fast(e, false, false, lp, strategy, emit, blk);
+			if (open && closed) cut(ci);
+			if (r == kFeFalse) break;
 		}
 	}
+	if (open) return;
 	// Flush() or Finish(): engine.Deflate(flush, finish) runs the function with canFlush = flush && inputOff == inputEnd
 	// (DeflaterEngine.cs:104-137) -- false as long as part of an undrained last SetInput is still outside the window
 	const bool finish = end_mode == 0;
 	for (;;) {
 		fe_fill_window(e);
-		if (fe_deflate_fast(e, e.inputOff == e.n, finish, lp, strategy, emit, block) == kFeFalse) break;
+		if (fe_deflate_fast(e, e.inputOff == e.n, finish, lp, strategy, emit, blk) == kFeFalse) break;
 	}
 	// (end_mode 1: the sync padding and the final empty static block that Finish() adds are appended by k_scan)
+}
+template <class EmitFn, class BlockFn>
+B200Z_HDN void fe_run(FastEngine &e, const LevelParams &lp, int strategy, int end_mode, EmitFn emit, BlockFn block,
+                      const uint32_t *cum = nullptr, int nchunks = 0, bool busy_last = true) {
+	fe_run(e, lp, strategy, end_mode, emit, block, [](int) {}, cum, nchunks, busy_last);
 }
 
 // ---- level 0: DeflaterEngine.DeflateStored (:614-649) --------------------------------------------------
@@ -598,13 +633,23 @@ struct StoredCarry {
 	int32_t strstart, blockStart;
 	uint32_t slides, inputOff;
 };
+// A stream going on from a carried state (a flush, or the cut of an open run): the state rebased (carry_rebase), and the
+// start_bias for stored_run when the data sits behind `hist` bytes of history in the slot -- the data starts at blockStart.
+B200Z_HD uint32_t stored_rebase(StoredCarry &c, uint32_t hist) {
+	carry_rebase(c.slides, c.inputOff);
+	return (uint32_t)(c.blockStart - 1) + 32768u * c.slides - hist;
+}
 // One segment of n bytes in `nchunks` SetInput calls (cum[] as for fe_run; stored-block boundaries depend on the schedule,
-// trap T9).  `carry`: in = the state a flushed earlier segment left (NULL: start of the stream, dict_len bytes of preset
-// dictionary in front); out = the state after this segment.  Block starts are stream offsets minus `start_bias`.
+// trap T9).  `carry`: in = the state a flushed earlier segment or the cut of an open run left (NULL: start of the stream,
+// dict_len bytes of preset dictionary in front); out = the state after this segment.  Block starts are stream offsets minus
+// `start_bias` (the stream offset of the first byte block starts are counted from, in the frame of carry_in's slides).
+// end_mode 3 (open run, as for fe_run): the BUSY_STATE loops only, over every call; `carry_out` is the state right behind
+// the last block that closed (the entry state if none did), *cut_call the call in whose Deflate() loop that happened.
+// Behind such a cut strstart may lie ahead of blockStart (a block ends at MAX_BLOCK_SIZE): those bytes are in the window.
 template <class BlockFn>
 inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn block, const uint32_t *cum = nullptr, int nchunks = 0,
                        const StoredCarry *carry_in = nullptr, StoredCarry *carry_out = nullptr, uint32_t start_bias = 0,
-                       bool busy_last = true) {
+                       bool busy_last = true, int *cut_call = nullptr) {
 	// host only: run when a plan is built
 	// dict_len: a preset dictionary in front of the n data bytes (SetDictionary leaves strstart = blockStart = 1 + length)
 	int strstart = 1 + (int)dict_len, blockStart = 1 + (int)dict_len, lookahead = 0;
@@ -615,7 +660,9 @@ inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn bloc
 		slides = carry_in->slides;
 		inputOff = carry_in->inputOff;
 	}
-	const uint32_t seg_base = inputOff;
+	const bool open = end_mode == 3;
+	// the data starts at blockStart; inputOff (lookahead is 0 between calls) is strstart - blockStart bytes further on
+	const uint32_t seg_base = inputOff - (uint32_t)(strstart - blockStart);
 	uint32_t vis = seg_base; // inputEnd: stream bytes handed over so far
 	const int kMaxBlock = 65531; // DeflaterConstants.MAX_BLOCK_SIZE
 	auto fill = [&]() {
@@ -631,6 +678,7 @@ inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn bloc
 			lookahead += (int)more;
 		}
 	};
+	bool closed = false;
 	auto stored = [&](bool flush, bool finish) -> bool {
 		if (!flush && lookahead == 0) return false;
 		strstart += lookahead;
@@ -645,19 +693,36 @@ inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn bloc
 			// window index w is stream byte w - 1 + 32768 * slides minus what the dictionary took (it is not stream data)
 			block((uint32_t)(blockStart - 1) + 32768u * slides - start_bias, (uint32_t)storedLength, lastBlock);
 			blockStart += storedLength;
+			closed = true;
 			return !(lastBlock || storedLength == 0);
 		}
 		return true;
 	};
+	auto save = [&](StoredCarry *c) {
+		if (!c) return;
+		c->strstart = strstart;
+		c->blockStart = blockStart;
+		c->slides = slides;
+		c->inputOff = inputOff;
+	};
+	save(carry_out);
+	if (cut_call) *cut_call = 0;
 	const int nc = nchunks > 0 ? nchunks : 1;
 	for (int ci = 0; ci < nc; ci++) {
 		vis = seg_base + (nchunks > 0 ? cum[ci] : n);
-		if (ci == nc - 1 && !busy_last) break;
+		if (ci == nc - 1 && !busy_last && !open) break;
 		for (;;) {
 			fill();
-			if (!stored(false, false)) break;
+			closed = false;
+			const bool more = stored(false, false);
+			if (open && closed) {
+				save(carry_out);
+				if (cut_call) *cut_call = ci;
+			}
+			if (!more) break;
 		}
 	}
+	if (open) return;
 	const bool finish = end_mode == 0;
 	for (;;) {
 		fill();
@@ -669,12 +734,7 @@ inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn bloc
 			if (!stored(inputOff == vis, true)) break;
 		}
 	}
-	if (carry_out) {
-		carry_out->strstart = strstart;
-		carry_out->blockStart = blockStart;
-		carry_out->slides = slides;
-		carry_out->inputOff = inputOff;
-	}
+	save(carry_out);
 }
 
 // ---- DeflaterHuffman.cs helpers ----------------------------------------------------------------

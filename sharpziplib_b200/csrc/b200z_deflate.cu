@@ -1087,7 +1087,7 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
                                             const uint32_t *__restrict__ hist, const LevelParams &lp, int strategy, int end_mode,
                                             int prev_entries, const uint32_t *__restrict__ sched, const uint32_t *__restrict__ sched_off,
                                             const int32_t *__restrict__ undrained, uint8_t *const *__restrict__ fstate, int cont,
-                                            int group) {
+                                            int group, uint2 *__restrict__ fcut) {
 	// prev[] is indexed by window position & 32767; when no stream of the batch is longer than prev_entries - 2 bytes the
 	// positions never reach prev_entries, so the table (and the CTA's shared-memory footprint) can be that much smaller
 	// and more CTAs share an SM.  (Plans that carry engine state between segments use whole tables.)
@@ -1115,17 +1115,25 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
 		if (lane == 0) fe_set_dictionary(e, hist[stream]); // preset dictionary in front of the data (0 = none)
 	}
 	e.coop = group ? 2 : 1;
-	// the SetInput schedule of the segment (fe_run in b200z_core.cuh is the serial statement of this loop)
+	// the SetInput schedule of the segment (fe_run in b200z_core.cuh is the serial statement of this loop, the open run's
+	// included)
 	const uint32_t *cum = sched + sched_off[stream];
 	const int nsched = (int)(sched_off[stream + 1] - sched_off[stream]);
 	const int nc = nsched > 0 ? nsched : 1;
-	const bool busy_last = undrained[stream] == 0;
-	uint32_t seg_base = 0, seg_len = 0;
+	const bool open = end_mode == B200Z_END_NONE;
+	const bool busy_last = undrained[stream] == 0 || open;
+	uint32_t seg_base = 0, seg_end = 0;
 	if (lane == 0) {
-		seg_base = e.inputOff;
-		seg_len = 32768u * e.slides - 1u - e.woff + e.slot_len - e.inputOff;
-		e.n = seg_base + (nsched > 0 ? cum[0] : seg_len);
+		seg_base = fe_stream_pos(e.slides, e.blockStart);
+		seg_end = 32768u * e.slides - 1u - e.woff + e.slot_len;
+		e.n = nsched > 0 ? seg_base + cum[0] : seg_end;
 	}
+	// an open run: the engine right behind the last block that closed is the next run's entry.  Tables and scalars are
+	// copied at every close that lies within one block's reach of the end of the input (the last one always does: behind it
+	// fewer than 16384 symbols of at most 258 bytes each follow, then less than MIN_LOOKAHEAD is left)
+	bool closed = false;
+	uint32_t cut_cov = 0, cut_call = 0;
+	if (open && lane == 0) fcut[stream] = make_uint2(0u, 0u);
 	uint32_t total = 0, nblk = 0;
 #ifdef B200Z_FAST_STATS
 	uint32_t st_steps = 0, st_pos = 0, st_lanes = 0;
@@ -1150,6 +1158,7 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
 					    bstart[nblk] = start;
 					    bptop[nblk] = ok ? 0xFFFFFFFEu : 0xFFFFFFFFu; // storedOffset sign decided by the engine (trap T4)
 					    ++nblk;
+					    closed = true;
 				    });
 				if (r != kFeNeedSlide && r != kFeGroup) in_deflate = false;
 			}
@@ -1195,6 +1204,28 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
 			if (r == kFeGroup) continue; // lane 0 goes on inside DeflateFast (in_deflate is still set)
 		}
 		r = __shfl_sync(0xffffffffu, r, 0);
+		if (open) {
+			// (a block closes only on lane 0's serial path: group steps stop one symbol short of a full block)
+			int snap = 0;
+			if (lane == 0 && closed) {
+				closed = false;
+				cut_cov = (uint32_t)e.blockStart + e.woff - hist[stream];
+				cut_call = (uint32_t)ci;
+				snap = e.slot_len - ((uint32_t)e.blockStart + e.woff) <= (uint32_t)(kBlockSyms * kMaxMatch + kMaxMatch + kMinMatch + 1);
+				if (snap) {
+					FastCarry c;
+					fe_save(e, c);
+					*reinterpret_cast<FastCarry *>(st + 131072) = c;
+				}
+			}
+			if (__shfl_sync(0xffffffffu, snap, 0)) {
+				__syncwarp();
+				uint4 *dst = reinterpret_cast<uint4 *>(st);
+				for (int i = lane; i < 65536 / 16; i += 32) dst[i] = reinterpret_cast<const uint4 *>(head)[i];
+				for (int i = lane; i < 65536 / 16; i += 32) dst[65536 / 16 + i] = reinterpret_cast<const uint4 *>(prev)[i];
+				__syncwarp();
+			}
+		}
 		if (r == kFeNeedSlide) {
 			// SlideWindow (DeflaterEngine.cs:441-462): scalars by lane 0, both tables by the warp
 			if (lane == 0) fe_slide_scalars(e);
@@ -1213,17 +1244,24 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
 		}
 		if (r == kFeFalse) {
 			if (phase == 1) break;
-			// chunk ci is drained ("needs input"): the next SetInput, or Flush()/Finish()
+			// chunk ci is drained ("needs input"): the next SetInput, or Flush()/Finish() (an open run ends here)
 			++ci;
 			if (ci < nc) {
 				if (lane == 0) e.n = seg_base + cum[ci];
 				if (ci == nc - 1 && !busy_last) phase = 1;
 			} else {
+				if (open) break;
 				phase = 1;
 			}
 		}
 	}
 	if (lane == 0) {
+		if (open) {
+			// the blocks in front of the cut are written; the last one ends where the next run's data starts
+			total = nblk * (uint32_t)kBlockSyms;
+			bstart[nblk] = cut_cov + hist[stream];
+			if (nblk) fcut[stream] = make_uint2(cut_cov, cut_call);
+		}
 		nsyms[stream] = total;
 		nblocks[stream] = nblk;
 #ifdef B200Z_FAST_STATS
@@ -1231,7 +1269,7 @@ __device__ __forceinline__ void fast_stream(const int stream, const int lane, ui
 		       st_steps, st_pos, st_steps ? (double)st_pos / st_steps : 0.0, st_steps ? (double)st_lanes / st_steps : 0.0, total);
 #endif
 	}
-	if (st) {
+	if (st && !open) {
 		// what the next segment of this stream starts from
 		__syncwarp();
 		uint4 *dst = reinterpret_cast<uint4 *>(st);
@@ -1255,7 +1293,7 @@ __global__ void __launch_bounds__(32)
            const uint32_t *__restrict__ hist, LevelParams lp, int strategy, int end_mode, int prev_entries,
            const uint32_t *__restrict__ sched, const uint32_t *__restrict__ sched_off, const int32_t *__restrict__ undrained,
            uint8_t *const *__restrict__ fstate, int cont, int group, int nstreams, uint16_t *__restrict__ head_pool,
-           uint32_t *__restrict__ counter) {
+           uint32_t *__restrict__ counter, uint2 *__restrict__ fcut) {
 	extern __shared__ __align__(16) uint8_t fsm[];
 	uint16_t *prev = reinterpret_cast<uint16_t *>(fsm);
 	// head_pool == nullptr: a batch of at most one stream per SM -- head[] sits behind prev[] in shared memory (one CTA per
@@ -1268,7 +1306,7 @@ __global__ void __launch_bounds__(32)
 		stream = __shfl_sync(0xffffffffu, stream, 0);
 		if (stream >= nstreams) break;
 		fast_stream(stream, lane, head, prev, in, sym, in_off, in_len, nsyms, nblocks, blk_off, blk_start, blk_ptop, hist, lp, strategy,
-		            end_mode, prev_entries, sched, sched_off, undrained, fstate, cont, group);
+		            end_mode, prev_entries, sched, sched_off, undrained, fstate, cont, group, fcut);
 		__syncwarp();
 	}
 }
@@ -1599,6 +1637,8 @@ struct DeflatePlan final : b200z_plan {
 	Slot<int32_t> o_undrained;
 	Slot<uint8_t *> o_fstate;
 	Slot<uint16_t> o_fhead;
+	Slot<uint2> o_fcut; // levels 1-4, open runs: per stream (covered, SetInput call) of the last cut, (0, 0) for none
+	std::vector<uint2> stored_cut; // level 0, open runs: the same, known when the plan is built
 };
 
 static int deflate_plan_build(DeflatePlan *p) {
@@ -1725,15 +1765,23 @@ static int deflate_plan_build(DeflatePlan *p) {
 				cin.slides = p->stored_state[i].slides;
 				cin.inputOff = p->stored_state[i].input_off;
 			}
+			// (the carried state fixes where the data starts: pos_base is not needed, and may have any size)
+			const uint32_t start_bias = cont ? stored_rebase(cin, (uint32_t)H) : 0u;
+			int cut_call = 0;
 			stored_run((uint32_t)(len - H), cont ? 0u : (uint32_t)H, p->end_mode, [&](uint32_t start, uint32_t blen, bool last) {
 				sblocks.push_back(StoredBlock{i, start, blen, last ? 1u : 0u, dst});
 				dst += 5 + (uint64_t)blen;
-			}, cum, nch, cont ? &cin : nullptr, &cout, cont ? (uint32_t)(p->pos_base[i] - H) : 0u, busy_last);
+			}, cum, nch, cont ? &cin : nullptr, &cout, start_bias, busy_last, &cut_call);
+			if (p->end_mode == B200Z_END_NONE) // the data in front of the last block's end; none written: the entry state
+				p->stored_cut.push_back(make_uint2(sblocks.empty() || sblocks.back().stream != i ? 0u
+				                                                       : sblocks.back().src + sblocks.back().len - (uint32_t)H,
+				                                   (uint32_t)cut_call));
 			// what the window took in: everything, except when Finish() right behind an undrained SetInput makes
 			// DeflateStored end the stream early (lastBlock = finish although input is left, DeflaterEngine.cs:629-641);
-			// TotalIn and the Adler-32 of the reference then cover the consumed bytes only, and so do ours
-			stored_taken[i] = (int64_t)(uint32_t)(cout.inputOff - (cont ? cin.inputOff : 0u));
-			if (p->stored_state) {
+			// TotalIn and the Adler-32 of the reference then cover the consumed bytes only, and so do ours.  (Behind the
+			// cut of an open run the data starts strstart - blockStart bytes in front of inputOff.)
+			stored_taken[i] = (int64_t)(uint32_t)(cout.inputOff - (cont ? cin.inputOff - (uint32_t)(cin.strstart - cin.blockStart) : 0u));
+			if (p->stored_state) { // (behind an open run: the state at its cut)
 				p->stored_state[i].strstart = cout.strstart;
 				p->stored_state[i].block_start = cout.blockStart;
 				p->stored_state[i].slides = cout.slides;
@@ -1807,6 +1855,7 @@ static int deflate_plan_build(DeflatePlan *p) {
 		p->o_fstate = ws.upload(fstate, 1);
 		p->o_fhead = ws.reserve<uint16_t>(p->fast_head_smem ? 128 : 32768ll * p->fast_ctas);
 		p->o_fcounter = ws.reserve<uint32_t>(64);
+		p->o_fcut = ws.reserve<uint2>(n + 1);
 	}
 	p->o_hist = ws.upload(hist32, 1);
 	p->o_bias = ws.upload(bias64, 1);
@@ -1834,7 +1883,7 @@ static int deflate_plan_build(DeflatePlan *p) {
 	B200Z_CUDA(cudaFuncSetAttribute(k_links, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinksSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileData + 2 * 2 * kTile));
 	p->launches = (lp.func == 2 ? 9 : (lp.func == 1 ? 4 : 2)) + (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // + one memset node
-	if (p->end_mode == B200Z_END_NONE) p->launches += 1 - (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // k_parse_cut, no checksum
+	if (p->end_mode == B200Z_END_NONE) p->launches += (lp.func == 2 ? 1 : 0) - (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // k_parse_cut, no checksum
 	return B200Z_OK;
 }
 
@@ -1850,10 +1899,15 @@ int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strateg
 	p->end_mode = end_mode;
 	p->in_len.assign(in_len, in_len + n);
 	if (end_mode == B200Z_END_NONE && level <= 4) {
-		// DeflateStored / DeflateFast carry window-relative tables across Deflate() calls that depend on the parse: a run
-		// cannot be resumed from a parse state alone
-		set_error("open runs (B200Z_END_NONE) are for levels 5-9");
-		return B200Z_E_UNSUPPORTED;
+		// DeflateStored / DeflateFast carry window-relative tables across Deflate() calls that depend on the parse: the cut
+		// of a run goes to the engine state the plan writes (b200z_history.engine_state / stored_state)
+		bool have = hist && n > 0 && (level == 0 ? hist->stored_state != nullptr : hist->engine_state != nullptr);
+		for (int i = 0; have && level >= 1 && i < n; i++) have = hist->engine_state[i] != nullptr;
+		if (!have) {
+			set_error("open runs (B200Z_END_NONE) at levels 0-4 need the engine state to write their cut into "
+			          "(b200z_history.engine_state / stored_state)");
+			return B200Z_E_UNSUPPORTED;
+		}
 	}
 	if (hist && n > 0 && level <= 4) {
 		// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
@@ -1916,7 +1970,8 @@ int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strateg
 			}
 			p->pos_base[i] = (hist->pos_base && hist->kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
 			p->bit_base[i] = hist->bit_base ? hist->bit_base[i] : 0;
-			if (p->pos_base[i] < H || (level <= 4 && p->pos_base[i] > 0xFFFF0000ll) || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
+			// (levels 0-4 keep positions relative to the carried engine state: carry_rebase)
+			if (p->pos_base[i] < H || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
 				set_error("stream %d: pos_base/bit_base", i);
 				return B200Z_E_ARG;
 			}
@@ -1978,6 +2033,7 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 		p->mark(s, "k_stored");
 		if (p->n_stored) k_stored<<<p->n_stored, 256, 0, s>>>(d_in, d_out, in_off, out_off, ws.at(p->o_stored));
 		k_set_results<<<(n + 127) / 128, 128, 0, s>>>(n, ws.at(p->o_slens), d_out_len, d_status, d_out_bits);
+		if (p->end_mode == B200Z_END_NONE) p->cut_ready = true;
 	} else {
 		if (do_encode) {
 			p->mark(s, "memset");
@@ -1990,7 +2046,8 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 			    d_in, sym, in_off, in_len, nsyms, nblocks, blk_off, blk_start, blk_ptop, hist, lp, p->strategy, p->end_mode,
 			    p->fast_prev_entries, ws.at(p->o_sched), ws.at(p->o_sched_off), ws.at(p->o_undrained), ws.at(p->o_fstate),
 			    p->hist_kind == B200Z_HIST_CONTINUE ? 1 : 0, fast_group_enabled(), n, p->fast_head_smem ? nullptr : ws.at(p->o_fhead),
-			    ws.at(p->o_fcounter));
+			    ws.at(p->o_fcounter), ws.at(p->o_fcut));
+			if (p->end_mode == B200Z_END_NONE) p->cut_ready = true;
 		} else {
 			if (do_search) {
 				p->mark(s, "k_links");
@@ -2079,11 +2136,33 @@ int deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry) {
 	return rc;
 }
 
+// levels 0-4: per stream (covered, SetInput call) of the last cut
+static int fast_cuts(DeflatePlan *p, std::vector<uint2> &v, cudaStream_t s) {
+	if (p->level == 0) {
+		v = p->stored_cut;
+		return B200Z_OK;
+	}
+	v.resize((size_t)p->n);
+	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->o_fcut), sizeof(uint2) * v.size(), cudaMemcpyDeviceToHost, s));
+	B200Z_CUDA(cudaStreamSynchronize(s));
+	return B200Z_OK;
+}
+
 int deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *next, cudaStream_t s) {
 	DeflatePlan *p = static_cast<DeflatePlan *>(plan);
 	if (p->end_mode != B200Z_END_NONE || !p->cut_ready) {
 		set_error("a cut is reported after a run of a B200Z_END_NONE plan");
 		return B200Z_E_STATE;
+	}
+	if (p->level <= 4) { // the engine state at the cut is in engine_state / stored_state; nothing is pending
+		std::vector<uint2> v;
+		const int rc = fast_cuts(p, v, s);
+		if (rc) return rc;
+		for (int i = 0; i < p->n; i++) {
+			covered[i] = v[i].x;
+			if (next) next[i] = b200z_parse_entry{0, kMinMatch - 1, 0};
+		}
+		return B200Z_OK;
 	}
 	std::vector<RoundRec> v((size_t)p->n);
 	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->o_cut), sizeof(RoundRec) * v.size(), cudaMemcpyDeviceToHost, s));
@@ -2096,6 +2175,19 @@ int deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *
 		next[i].match_len = (int32_t)v[i].mlen;
 		next[i].match_dist = v[i].mlen >= (uint32_t)kMinMatch ? pos - (int64_t)v[i].mstart : 0;
 	}
+	return B200Z_OK;
+}
+
+int deflate_plan_get_cut_call(b200z_plan *plan, int32_t *call, cudaStream_t s) {
+	DeflatePlan *p = static_cast<DeflatePlan *>(plan);
+	if (p->end_mode != B200Z_END_NONE || !p->cut_ready || p->level > 4) {
+		set_error("a cut's SetInput call is reported after a run of a level 0-4 B200Z_END_NONE plan");
+		return B200Z_E_STATE;
+	}
+	std::vector<uint2> v;
+	const int rc = fast_cuts(p, v, s);
+	if (rc) return rc;
+	for (int i = 0; i < p->n; i++) call[i] = (int32_t)v[i].y;
 	return B200Z_OK;
 }
 

@@ -78,9 +78,9 @@ static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const ui
 // =====================================================================================================
 // Streaming handles
 // =====================================================================================================
-// Levels 5-9 compress a long stream in open runs (B200Z_END_NONE) of this many new bytes, plus what the run in front left
-// behind its cut: a plan's workspace grows with its input (about 3.7 GB for 256 MiB), and the output flows while input
-// arrives.  A segment up to this size runs as one plan, as it always has.
+// A long stream is compressed in open runs (B200Z_END_NONE) of this many new bytes, plus what the run in front left behind
+// its cut: a plan's workspace grows with its input (about 3.7 GB for 256 MiB at levels 5-9), the host holds no more than
+// that, and the output flows while input arrives.  A segment up to this size runs as one plan, as it always has.
 constexpr int64_t kOpenRunBytes = 256ll << 20;
 constexpr b200z_parse_entry kCleanEntry = {0, kMinMatch - 1, 0};
 
@@ -98,7 +98,7 @@ struct DeflaterH {
 	bool dict_set = false, deflate_called = false, started = false;
 	uint32_t dict_adler = 0;
 	std::vector<uint8_t> input;    // everything SetInput handed over and not yet compressed
-	// levels 5-9: the parse state the next run starts from, the bytes at the front of `input` that the last open run saw
+	// the parse state the next run starts from (levels 5-9), the bytes at the front of `input` that the last open run saw
 	// but left behind its cut, and whether that run's output is still being handed out
 	b200z_parse_entry entry = kCleanEntry;
 	int64_t carried = 0;
@@ -108,8 +108,9 @@ struct DeflaterH {
 	HostBits tail;                 // sub-byte tail carried between device runs
 	int64_t total_in = 0, total_out = 0;
 	uint32_t adler = 1;
-	// levels 0-4 depend on the call pattern (trap T9) and keep engine state across Flush(): the sizes of the SetInput calls
-	// since the last run, whether Deflate() was called behind the last of them, and what the engines carry
+	// levels 0-4 depend on the call pattern (trap T9) and keep engine state across Flush() and cuts: the sizes of the SetInput
+	// calls in `input` (behind a cut the first is the rest of the call the cut fell into), whether Deflate() was called behind
+	// the last of them, and what the engines carry
 	std::vector<int64_t> chunks;
 	bool undrained = false;
 	b200z_stored_state sstate = {0, 0, 0, 0}; // level 0 (DeflateStored)
@@ -143,17 +144,17 @@ static void deflater_header(DeflaterH *d) {
 	d->header_done = true;
 }
 
-static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
-	// compresses the first `len` bytes of d->input as the next segment of the stream; END_FLUSH keeps the stream open and may
-	// end inside a byte; END_NONE (levels 5-9) writes the blocks that closed and keeps the bytes behind them for the next run
+static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len, int32_t n_chunks) {
+	// compresses the first `len` bytes of d->input (levels 0-4: the first n_chunks SetInput calls) as the next segment of the
+	// stream; END_FLUSH keeps the stream open and may end inside a byte; END_NONE writes the blocks that closed and keeps the
+	// bytes behind them for the next run
 	const bool open = end_mode == B200Z_END_NONE;
 	const int64_t H = (int64_t)d->history.size();
 	const bool continuing = d->started; // an earlier segment (possibly empty) has been emitted
 	b200z_history hs;
 	memset(&hs, 0, sizeof hs);
-	const int32_t n_chunks = (int32_t)d->chunks.size();
 	const int64_t *chunk_ptr = d->chunks.data();
-	const int32_t undrained = (d->undrained && n_chunks > 0) ? 1 : 0;
+	const int32_t undrained = (d->undrained && n_chunks == (int32_t)d->chunks.size() && n_chunks > 0 && !open) ? 1 : 0;
 	void *fstate_ptr = nullptr;
 	if (d->level <= 4) {
 		hs.chunk_count = &n_chunks;
@@ -176,7 +177,9 @@ static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
 	hs.pos_base = &pos_base;
 	hs.bit_base = &bit_base;
 	hs.hist_mask = &mask;
-	const uint32_t stored_before = d->sstate.input_off;
+	// level 0: the state as the plan rebases it, for the bytes a closing run takes (see stored_run)
+	b200z_stored_state sbefore = d->sstate;
+	if (continuing) carry_rebase(sbefore.slides, sbefore.input_off);
 	b200z_plan *plan = nullptr;
 	int rc = b200z_deflate_plan_create_ex(1, &len, d->level, d->strategy, d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB, end_mode,
 	                                      (hs.kind != B200Z_HIST_NONE || d->level <= 4) ? &hs : nullptr, &plan);
@@ -199,8 +202,10 @@ static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
 	}
 	int64_t covered = len; // bytes of input this run is done with
 	b200z_parse_entry next = kCleanEntry;
+	int32_t cut_call = 0;
 	if (!rc && open) {
-		rc = b200z_deflate_plan_get_cut(plan, &covered, &next, nullptr);
+		rc = b200z_deflate_plan_get_cut(plan, &covered, d->level >= 5 ? &next : nullptr, nullptr);
+		if (!rc && d->level <= 4) rc = b200z_deflate_plan_get_cut_call(plan, &cut_call, nullptr);
 		if (!rc && covered <= 0) { // (a run of more than 16384 * 258 + 262 bytes always closes a block)
 			set_error("open run of %lld bytes closed no block", (long long)len);
 			rc = B200Z_E_INTERNAL;
@@ -226,8 +231,11 @@ static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
 		d->tail.bits = d->tail.count ? (seg[(size_t)whole] & ((1u << d->tail.count) - 1u)) : 0u;
 		if (end_mode == B200Z_END_FINISH) d->tail.align(d->pending); // FINISHING_STATE: AlignToByte (:507)
 		if (!d->raw && !open) d->adler = r.check[0];
-		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run)
-		d->total_in += d->level == 0 ? (int64_t)(uint32_t)(d->sstate.input_off - stored_before) : covered;
+		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run;
+		// the data starts strstart - block_start bytes in front of the state's input_off)
+		d->total_in += (d->level == 0 && !open)
+		                   ? (int64_t)(uint32_t)(d->sstate.input_off - sbefore.input_off) + (sbefore.strstart - sbefore.block_start)
+		                   : covered;
 		d->started = true;
 		// every position in front of a cut went through InsertString; a flush leaves the last two out
 		deflater_remember(d, d->input.data(), (size_t)covered, open ? 0 : 2);
@@ -237,28 +245,52 @@ static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len) {
 		if (!open) {
 			d->chunks.clear();
 			d->undrained = false;
+		} else if (d->level <= 4) {
+			// the next run's schedule: the rest of the call the cut fell into, then the calls behind it
+			int64_t end = 0;
+			for (int32_t k = 0; k <= cut_call; k++) end += d->chunks[(size_t)k];
+			d->chunks.erase(d->chunks.begin(), d->chunks.begin() + cut_call);
+			d->chunks[0] = end - covered;
 		}
 	}
 	b200z_plan_destroy(plan);
 	return rc;
 }
 
-// Levels 5-9: while more than one run's worth of input is buffered, the front of it is compressed in open runs and their
-// output is due at once.  Each run takes the bytes its predecessor left behind the cut plus at most kOpenRunBytes more,
-// so it is longer than a block can be and always ends in a cut: no run is repeated on the same bytes.
+// While more than one run's worth of input is buffered, the front of it is compressed in open runs and their output is due
+// at once.  Each run takes the bytes its predecessor left behind the cut plus at most kOpenRunBytes more, so it is longer
+// than a block can be and always ends in a cut: no run is repeated on the same bytes.  Levels 0-4 take whole SetInput
+// calls whose Deflate() already ran (enough of them to close a block, however long the last one is): a call that Flush() /
+// Finish() follows directly stays with the closing run (b200z_history.undrained_last).
 static int deflater_open_runs(DeflaterH *d) {
-	while (d->level >= 5 && (int64_t)d->input.size() > kOpenRunBytes) {
+	for (;;) {
+		const bool fast = d->level <= 4;
+		int32_t ncalls = (int32_t)d->chunks.size() - ((fast && d->undrained && !d->chunks.empty()) ? 1 : 0);
+		int64_t avail = (int64_t)d->input.size();
+		if (fast) {
+			avail = 0;
+			for (int32_t k = 0; k < ncalls; k++) avail += d->chunks[(size_t)k];
+		}
+		if (avail <= kOpenRunBytes) return B200Z_OK;
+		int64_t len = std::min<int64_t>(avail, d->carried + kOpenRunBytes);
+		if (fast) {
+			int64_t sum = 0;
+			int32_t k = 0;
+			// (more than one block's reach behind the carried bytes: the run closes a block)
+			const int64_t least = d->carried + (int64_t)kBlockSyms * kMaxMatch + kMaxMatch + kMinMatch + 1;
+			while (k < ncalls && (sum < least || sum + d->chunks[(size_t)k] <= len)) sum += d->chunks[(size_t)k++];
+			len = sum;
+			ncalls = k;
+		}
 		if (d->pending_pos == d->pending.size()) {
 			d->pending.clear();
 			d->pending_pos = 0;
 		}
 		deflater_header(d);
-		const int64_t len = std::min<int64_t>((int64_t)d->input.size(), d->carried + kOpenRunBytes);
-		int rc = deflater_run_device(d, B200Z_END_NONE, len);
+		int rc = deflater_run_device(d, B200Z_END_NONE, len, ncalls);
 		if (rc) return rc;
 		d->draining = true;
 	}
-	return B200Z_OK;
 }
 
 // ---- Inflater handle ----------------------------------------------------------------------------------
@@ -516,16 +548,8 @@ int b200z_deflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 		set_error("buffer/count");
 		return B200Z_E_ARG;
 	}
-	// one plan slot addresses 4 GiB - 64 KiB (32-bit positions, the window phase included): refuse what could not be
-	// compressed instead of accepting it and failing at Flush() / Finish().  Levels 5-9 run long input in open runs, and
-	// their plans take a stream position of any size.
-	if (d->level <= 4 &&
-	    ((int64_t)d->input.size() + len + 32768 > 0xFFFF0000ll || d->window_seen + (int64_t)d->input.size() + len > 0xFFFF0000ll)) {
-		set_error("Deflater handle: more than 4 GiB - 64 KiB in one stream (TotalIn %lld, %lld buffered, %d more): use several "
-		          "streams or the batch API",
-		          (long long)d->total_in, (long long)d->input.size(), len);
-		return B200Z_E_UNSUPPORTED;
-	}
+	// (no length limit: Deflate() runs long input in open runs, so a closing run holds at most what the last one carried,
+	// kOpenRunBytes and one SetInput of at most 2^31 - 1 bytes, and plans take a stream position of any size)
 	if (len > 0) d->flushed_once = false;
 	d->input.insert(d->input.end(), buf, buf + len);
 	if (len > 0) {
@@ -577,7 +601,7 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 					d->tail.align(d->pending);
 				}
 			} else {
-				int rc = deflater_run_device(d, B200Z_END_FINISH, (int64_t)d->input.size());
+				int rc = deflater_run_device(d, B200Z_END_FINISH, (int64_t)d->input.size(), (int32_t)d->chunks.size());
 				if (rc) return rc;
 			}
 			if (!d->raw) {
@@ -589,7 +613,7 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 			d->finished = true;
 		} else {
 			// sync flush (level 0 skips the padding, :488)
-			int rc = deflater_run_device(d, B200Z_END_FLUSH, (int64_t)d->input.size());
+			int rc = deflater_run_device(d, B200Z_END_FLUSH, (int64_t)d->input.size(), (int32_t)d->chunks.size());
 			if (rc) return rc;
 			d->flushed_once = true;
 			d->flushing = false;

@@ -200,6 +200,7 @@ int deflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t
                      uint32_t *d_check, int64_t *d_out_bits, cudaStream_t s, int stages);
 int deflate_plan_set_entry(b200z_plan *p, const b200z_parse_entry *entry);
 int deflate_plan_get_cut(b200z_plan *p, int64_t *covered, b200z_parse_entry *next, cudaStream_t s);
+int deflate_plan_get_cut_call(b200z_plan *p, int32_t *call, cudaStream_t s);
 int inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int wrap, const int64_t *dict_len,
                         b200z_plan **out);
 int inflate_plan_set_start_bits(b200z_plan *p, const int32_t *start_bit);
