@@ -91,20 +91,22 @@ __device__ __forceinline__ uint32_t sub_word(const uint32_t *te, uint32_t w) { /
 constexpr int kAesThreads = 256;
 constexpr int kAesBlocksPerThread = 4;
 constexpr int kAesTile = kAesThreads * kAesBlocksPerThread * 16; // bytes of keystream per CTA and grid step
+constexpr int kAesMaxTiles = 1024;                                 // CTAs per stream; longer streams loop (16 MiB per step)
 
-// grid (tiles, streams).  keys: per stream 2 * key_bytes + 2 bytes (key1 | key2 | verifier).
+// grid (streams, tiles): streams on x (up to 2^31 - 1 of them), at most kAesMaxTiles tiles on y.  keys: per stream
+// 2 * key_bytes + 2 bytes (key1 | key2 | verifier).
 __global__ void __launch_bounds__(kAesThreads)
     k_aes_ctr(const uint8_t *__restrict__ in, uint8_t *__restrict__ out, const int64_t *__restrict__ off,
               const int64_t *__restrict__ len, const uint8_t *__restrict__ keys, int key_bytes, const AesState *__restrict__ state,
               int hashed) {
 	__shared__ uint32_t s_te[256];
 	__shared__ uint32_t s_rk[60];
-	const int stream = blockIdx.y;
+	const int stream = blockIdx.x;
 	const int64_t n = len[stream];
 	// stream position of this call's first byte: the state's count, which the HMAC kernel has already advanced when it ran first
 	const uint64_t start = state[stream].bytes - (hashed ? (uint64_t)(n > 0 ? n : 0) : 0u);
 	const uint64_t first_blk = start >> 4, last_blk = (start + (uint64_t)n + 15) >> 4;
-	if (n <= 0 || first_blk + (uint64_t)blockIdx.x * (kAesTile / 16) >= last_blk) return;
+	if (n <= 0 || first_blk + (uint64_t)blockIdx.y * (kAesTile / 16) >= last_blk) return;
 	s_te[threadIdx.x] = c_te0[threadIdx.x];
 	__syncthreads();
 	const int nk = key_bytes / 4, rounds = nk + 6;
@@ -128,7 +130,7 @@ __global__ void __launch_bounds__(kAesThreads)
 	__syncthreads();
 	const uint8_t *src = in + off[stream];
 	uint8_t *dst = out + off[stream];
-	for (uint64_t tb = first_blk + (uint64_t)blockIdx.x * (kAesTile / 16); tb < last_blk; tb += (uint64_t)gridDim.x * (kAesTile / 16)) {
+	for (uint64_t tb = first_blk + (uint64_t)blockIdx.y * (kAesTile / 16); tb < last_blk; tb += (uint64_t)gridDim.y * (kAesTile / 16)) {
 #pragma unroll
 		for (int j = 0; j < kAesBlocksPerThread; j++) {
 			const uint64_t kb = tb + (uint64_t)j * kAesThreads + threadIdx.x;
@@ -352,9 +354,9 @@ __global__ void __launch_bounds__(64)
     k_pbkdf2(const uint8_t *__restrict__ pw, const int64_t *__restrict__ pw_off, const uint8_t *__restrict__ salts, int key_bytes,
              int rounds, uint8_t *__restrict__ out, int n) {
 	const int nblk = (2 * key_bytes + 2 + 19) / 20;
-	const int t = blockIdx.x * blockDim.x + threadIdx.x;
-	if (t >= n * nblk) return;
-	const int stream = t / nblk, blk = t % nblk + 1;
+	const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= (int64_t)n * nblk) return;
+	const int stream = (int)(t / nblk), blk = (int)(t % nblk) + 1;
 	const uint8_t *p = pw + pw_off[stream];
 	const int pn = (int)(pw_off[stream + 1] - pw_off[stream]);
 	uint8_t kbuf[64];
@@ -479,8 +481,10 @@ static int aes_launch(const uint8_t *d_in, uint8_t *d_out, const int64_t *d_off,
 	if (n <= 0) return B200Z_OK;
 	int64_t tiles = (max_len + 16 + kAesTile - 1) / kAesTile;
 	if (tiles < 1) tiles = 1;
-	if (tiles > 1024) tiles = 1024;
-	const dim3 grid((unsigned)tiles, (unsigned)n);
+	if (tiles > kAesMaxTiles) tiles = kAesMaxTiles;
+	// any int32 stream count fits gridDim.x and the tiles fit gridDim.y, so neither launch can be refused for its shape after
+	// the other one has run and advanced the carried state
+	const dim3 grid((unsigned)n, (unsigned)tiles);
 	const int hb = (n + 63) / 64;
 	if (write_mode) {
 		k_aes_ctr<<<grid, kAesThreads, 0, s>>>(d_in, d_out, d_off, d_len, d_keys, key_bytes, d_state, 0);
@@ -533,7 +537,7 @@ int b200z_aes_derive_keys(const uint8_t *passwords, const int64_t *pw_off, const
 	B200Z_CUDA(cudaMemcpy(d_off, pw_off, 8ull * (n + 1), cudaMemcpyHostToDevice));
 	B200Z_CUDA(cudaMemcpy(d_salt, salts, (size_t)sn, cudaMemcpyHostToDevice));
 	const int nblk = (2 * key_bytes + 2 + 19) / 20;
-	k_pbkdf2<<<(n * nblk + 63) / 64, 64, 0, 0>>>(d_pw, d_off, d_salt, key_bytes, 1000, d_out, n);
+	k_pbkdf2<<<(unsigned)(((int64_t)n * nblk + 63) / 64), 64, 0, 0>>>(d_pw, d_off, d_salt, key_bytes, 1000, d_out, n);
 	B200Z_CUDA(cudaGetLastError());
 	B200Z_CUDA(cudaMemcpy(keys_out, d_out, (size_t)on, cudaMemcpyDeviceToHost));
 	return B200Z_OK;
