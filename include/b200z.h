@@ -193,6 +193,22 @@ int b200z_inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit
  * b200z_plan_data_offset(i) stays.  This is how the Inflater handle keeps ONE plan between SetInput calls. */
 int b200z_inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, const int64_t *dict_len);
 int b200z_plan_get_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_pos, void *cuda_stream);
+/* Resuming inside a Huffman block: the decoder carries the window, the bit position and the block's code tables, and
+ * the tables come from the block's header.  So a raw inflate plan can enter a stream in mid-block: stream i's slot holds
+ * the window image (as the dictionary), a copy of the block header starting at bit start_bit[i] (0..7) of its first byte,
+ * then the compressed bytes from the resume point on.  The decoder reads the header (tables, BFINAL) and goes on at bit
+ * skip_bit[i] of the slot, past the rest of the header copy's last byte; the run's output starts with the symbol there.
+ * skip_bit[i] = 0 is no jump (b200z_inflate_plan_set_start_bits).  A stored-block header, or a header that ends behind
+ * skip_bit[i], makes the stream's status B200Z_E_ARG.  Host arrays of n entries. */
+int b200z_inflate_plan_set_resume(b200z_plan *plan, const int32_t *start_bit, const int64_t *skip_bit);
+/* Where each stream of the last run can be resumed (bits from the first compressed byte of the slot): hdr_bit[i] the
+ * header of the block it stopped in (= the restart point), body_bit[i] where that header ends, sym_bit[i] the first
+ * symbol not decoded, out_pos[i] the output bytes in front of it.  Inside a block only when the stream stopped in a
+ * Huffman block with B200Z_E_NEED_INPUT (or B200Z_E_NOMEM: the serial kernel stops between two symbols); in a header, a
+ * stored block or any other case sym_bit == body_bit == hdr_bit and out_pos is the restart point's.  Synchronises the
+ * stream like get_restart_points. */
+int b200z_plan_get_resume_points(b200z_plan *plan, int64_t *hdr_bit, int64_t *body_bit, int64_t *sym_bit, int64_t *out_pos,
+                                 void *cuda_stream);
 /* Diagnostics of the last run of an inflate plan (synchronises `stream`): v[0] positions that passed the finder's first
  * two stages, v[1] segments decoded (stream starts + block-header candidates), v[2] round slots taken, v[3] Huffman blocks
  * decoded, v[4] rounds, v[5] speculative passes over them, v[6] streams handed back to the serial kernel, v[7] 1 if the
@@ -326,6 +342,10 @@ int b200z_inflater_remaining_input(void *h, int32_t *v);                        
 int b200z_inflater_total_in(void *h, int64_t *v);                                   /* :862 */
 int b200z_inflater_total_out(void *h, int64_t *v);                                  /* :848 */
 int b200z_inflater_adler(void *h, uint32_t *v);                                     /* :823 */
+/* Diagnostics of the handle since create / Reset (mirrors nothing in the reference): v[0] device runs, v[1] output bytes
+ * the runs produced (bytes decoded twice counted twice), v[2] the most compressed bytes the handle held at once (input
+ * kept + header copy), v[3] the most output bytes it held at once (undelivered output + window).  cap entries at most. */
+int b200z_inflater_get_stats(void *h, int64_t *v, int32_t cap);
 
 /* ---- Entry ciphers applied to compressed bytes (SURVEY.md row f4) ---------------------------------------------------
  * Encryption/ZipAESTransform.cs (WinZip AES: AES-CTR + HMAC-SHA1, keys by PBKDF2) and Encryption/PkzipClassic.cs, the

@@ -76,6 +76,8 @@ _SIGS = {
     "b200z_inflate_plan_create_ex": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]),
     "b200z_inflate_plan_set_start_bits": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200z_plan_get_restart_points": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_inflate_plan_set_resume": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_plan_get_resume_points": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_inflate_plan_set_lengths": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_plan_get_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "b200z_plan_data_offset": (C.c_int64, [C.c_void_p, C.c_int32]),
@@ -154,6 +156,7 @@ _SIGS = {
     "b200z_inflater_total_in": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "b200z_inflater_total_out": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "b200z_inflater_adler": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32)]),
+    "b200z_inflater_get_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
 }
 
 EXPORTS = tuple(sorted(_SIGS))

@@ -205,6 +205,15 @@ class InflatePlan(_Plan):
         assert sb.size == self.n
         _lib.raise_for(_lib.lib().b200z_inflate_plan_set_start_bits(self._h, sb.ctypes.data))
 
+    def set_resume(self, start_bits, skip_bits):
+        """Raw plans: stream i enters a Huffman block in its middle.  Its slot holds the block's header from bit start_bits[i]
+        (0..7) of its first compressed byte, then the compressed bytes from the resume point on; decoding goes on at bit
+        skip_bits[i] of the slot (0: no jump, a plain start bit).  The window image is passed as the dictionary."""
+        sb = np.ascontiguousarray(start_bits, dtype=np.int32)
+        kb = np.ascontiguousarray(skip_bits, dtype=np.int64)
+        assert sb.size == self.n and kb.size == self.n
+        _lib.raise_for(_lib.lib().b200z_inflate_plan_set_resume(self._h, sb.ctypes.data, kb.ctypes.data))
+
     def stats(self, stream=None):
         """diagnostics of the last run (b200z_plan_get_stats): finder survivors, segments, round slots, blocks, rounds, passes,
         streams handed back to the serial kernel, pipeline in use"""
@@ -224,6 +233,17 @@ class InflatePlan(_Plan):
         pos = np.zeros(self.n, dtype=np.int64)
         _lib.raise_for(_lib.lib().b200z_plan_get_restart_points(self._h, bit.ctypes.data, pos.ctypes.data, s.cuda_stream))
         return bit, pos
+
+    def resume_points(self, stream=None):
+        """(hdr_bit, body_bit, sym_bit, out_pos) int64 arrays of the last run (bits from the first compressed byte of the
+        slot): the header of the block each stream stopped in, where that header ends, the first symbol not decoded and the
+        output bytes in front of it.  Inside the block only for a stream that stopped in a Huffman block; otherwise the three
+        bits are the restart point.  Synchronises the stream."""
+        import torch
+        s = stream if stream is not None else torch.cuda.current_stream()
+        v = [np.zeros(self.n, dtype=np.int64) for _ in range(4)]
+        _lib.raise_for(_lib.lib().b200z_plan_get_resume_points(self._h, *(a.ctypes.data for a in v), s.cuda_stream))
+        return tuple(v)
 
 
 class Pipeline:

@@ -202,3 +202,10 @@ class Inflater:
         v = C.c_uint32(0)
         _lib.raise_for(_lib.lib().b200z_inflater_adler(self._h, C.byref(v)))
         return v.value
+
+    def stats(self):
+        """diagnostics since construction / Reset (b200z_inflater_get_stats; not in the reference): device runs, output bytes
+        the runs produced (re-decoded bytes counted again), most compressed and most output bytes held at once"""
+        v = np.zeros(4, dtype=np.int64)
+        _lib.raise_for(_lib.lib().b200z_inflater_get_stats(self._h, v.ctypes.data, 4))
+        return dict(zip(("runs", "decoded", "max_comp_held", "max_out_held"), (int(x) for x in v)))

@@ -349,6 +349,25 @@ int b200z_inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit
 	return inflate_plan_set_start_bits(plan, start_bit);
 }
 
+int b200z_inflate_plan_set_resume(b200z_plan *plan, const int32_t *start_bit, const int64_t *skip_bit) {
+	DeviceGuard guard(plan ? plan->device : -1);
+	if (!plan || plan->kind != 1 || (plan->n > 0 && (!start_bit || !skip_bit))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	if (plan->wrap != B200Z_WRAP_RAW) {
+		set_error("resume points are for raw streams");
+		return B200Z_E_ARG;
+	}
+	for (int i = 0; i < plan->n; i++) {
+		if (start_bit[i] < 0 || start_bit[i] > 7 || skip_bit[i] < 0 || skip_bit[i] > 0x7FFFFFFF8ll) {
+			set_error("stream %d: start bit %d (0..7), skip bit %lld", i, start_bit[i], (long long)skip_bit[i]);
+			return B200Z_E_ARG;
+		}
+	}
+	return inflate_plan_set_resume(plan, start_bit, skip_bit);
+}
+
 int b200z_inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, const int64_t *dict_len) {
 	DeviceGuard guard(plan ? plan->device : -1);
 	if (!plan || plan->kind != 1 || (plan->n > 0 && !comp_len)) {
@@ -366,6 +385,17 @@ int b200z_plan_get_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_p
 	}
 	if (plan->n == 0) return B200Z_OK;
 	return inflate_plan_restart_points(plan, bit, out_pos, (cudaStream_t)cuda_stream);
+}
+
+int b200z_plan_get_resume_points(b200z_plan *plan, int64_t *hdr_bit, int64_t *body_bit, int64_t *sym_bit, int64_t *out_pos,
+                                 void *cuda_stream) {
+	DeviceGuard guard(plan ? plan->device : -1);
+	if (!plan || plan->kind != 1 || (plan->n > 0 && (!hdr_bit || !body_bit || !sym_bit || !out_pos))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	if (plan->n == 0) return B200Z_OK;
+	return inflate_plan_resume_points(plan, hdr_bit, body_bit, sym_bit, out_pos, (cudaStream_t)cuda_stream);
 }
 
 int b200z_plan_get_stats(b200z_plan *plan, uint32_t *v, int32_t cap, void *cuda_stream) {

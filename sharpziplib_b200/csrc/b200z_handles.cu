@@ -294,25 +294,31 @@ static int deflater_open_runs(DeflaterH *d) {
 }
 
 // ---- Inflater handle ----------------------------------------------------------------------------------
-// The reference's Inflater is a mode machine that stops at any bit and resumes (Inflater.cs:73-86, :429-552).  The kernel
-// decodes whole plans, so the handle resumes at BLOCK granularity: k_inflate reports the last block header it reached
-// (bit position, output position -- the "restart point"); when more input arrives decoding continues from that header
-// with the last 32 KiB of output in front of it as the window image.  Bytes of a block that was only partly available
-// are decoded again by the next run (they were already delivered; the new run's output replaces them byte for byte).
-// Work is linear in the stream for any SetInput granularity as long as blocks are bounded (the reference's own Deflater
-// cuts a block every 16384 symbols), and the handle holds one block of input / output plus the window, not the stream.
+// The reference's Inflater is a mode machine that stops at any bit and resumes (Inflater.cs:73-86, :429-552).  The kernels
+// decode whole plans and report where a stream that ran out of input can be resumed (b200z_plan_get_resume_points): inside
+// a Huffman block at the first symbol not decoded, otherwise at the block header it stopped in.  Between SetInput calls the
+// handle keeps the window (the last 32 KiB of output), a copy of the current block's header when it stopped inside the
+// block, and the compressed bytes from the resume point on; the next run enters the block through the header copy
+// (b200z_inflate_plan_set_resume) and appends its output.  A stream stops inside a Huffman block only a symbol (at most 48
+// bits) short of the input's end, in a header at most a header (under 600 bytes) short, and in front of a stored block at
+// most 65535 + 5 bytes short: that, one header copy and the last SetInput are all the compressed bytes the handle holds,
+// whatever the block size, and no byte is decoded twice.
 struct InflaterH {
 	bool raw = false;
-	std::vector<uint8_t> input; // compressed bytes from absolute offset in_base on (what lies in front of the restart point is dropped)
+	std::vector<uint8_t> input; // compressed bytes from absolute offset in_base on (what lies in front of the resume point is dropped)
 	int64_t in_base = 0, in_total = 0; // in_total = bytes handed over since Reset = in_base + input.size()
 	bool new_input = false;
 	bool finished = false;
 	bool need_dict = false;
 	bool header_done = false;
+	bool raw_done = false;     // the final block has ended; a zlib stream awaits its trailer at trailer_at
+	int64_t trailer_at = 0;
 	uint32_t read_adler = 0;   // DICTID from the header (Inflater.readAdler)
 	int64_t raw_off = 0;       // where the raw deflate data starts (behind the zlib header)
-	int64_t rs_bit = 0;        // restart point: bit offset from raw_off of the block header decoding continues at
-	int64_t rs_out = 0;        //                output position of that header
+	int64_t rs_bit = 0;        // resume point: bit offset from raw_off where decoding goes on -- a block header, or a symbol of
+	int64_t rs_out = 0;        //   the block whose header `hdr` holds; output position there
+	std::vector<uint8_t> hdr;  // that block's header bytes, from bit hdr_sbit of hdr[0] on (empty: rs_bit is a header)
+	int32_t hdr_sbit = 0;
 	std::vector<uint8_t> window; // last <= 32768 bytes of (dictionary ++ output[0, rs_out)): OutputWindow's contents there
 	uint32_t run_adler = 1;    // Adler-32 of output[0, rs_out)
 	std::vector<uint8_t> output; // decoded bytes from output position out_base on (delivered bytes in front of rs_out are dropped)
@@ -322,6 +328,7 @@ struct InflaterH {
 	uint32_t adler = 1;
 	int error = 0;
 	std::string error_msg;
+	int64_t stats[4] = {0, 0, 0, 0}; // b200z_inflater_get_stats
 	Staging st;
 	// one plan per handle, created for capacities and run below them (b200z_inflate_plan_set_lengths): a SetInput + Inflate
 	// pair costs the copies and the kernels, no allocation
@@ -329,91 +336,122 @@ struct InflaterH {
 	int64_t plan_comp_cap = 0, plan_out_cap = 0;
 	~InflaterH() { b200z_plan_destroy(plan); }
 	int64_t out_total() const { return out_base + (int64_t)output.size(); }
+	void note_held() {
+		stats[2] = std::max(stats[2], (int64_t)(input.size() + hdr.size()));
+		stats[3] = std::max(stats[3], (int64_t)(output.size() + window.size()));
+	}
 };
 
-// decodes from the restart point to the end of what is available; fills output / consumed / finished and moves the
-// restart point forward
-static int inflater_run_device(InflaterH *d) {
-	const int64_t slice_abs = d->raw_off + (d->rs_bit >> 3); // absolute offset of the first compressed byte of this run
-	const int32_t sbit = (int32_t)(d->rs_bit & 7);
-	const int64_t avail = d->in_total - slice_abs;
-	if (avail < 0 || slice_abs < d->in_base) {
-		set_error("inflater restart point outside the kept input");
-		return B200Z_E_INTERNAL;
+// checksum and window advance over the next n bytes of output, which start at output position rs_out
+static int inflater_advance(InflaterH *d, int64_t n) {
+	const uint8_t *seg = d->output.data() + (d->rs_out - d->out_base);
+	if (!d->raw && n > 0) {
+		int rc = b200z_adler32(seg, n, &d->run_adler);
+		if (rc) return rc;
 	}
-	int64_t cap = avail * 8 + 65536;
+	if (n >= 32768) d->window.assign(seg + n - 32768, seg + n);
+	else {
+		d->window.insert(d->window.end(), seg, seg + n);
+		if (d->window.size() > 32768) d->window.erase(d->window.begin(), d->window.end() - 32768);
+	}
+	d->rs_out += n;
+	return B200Z_OK;
+}
+
+// output in front of both the resume point and the delivery position is not needed any more.  Dropped once per run (a
+// reader has usually taken everything by then): erasing it on every Inflate() would move the rest of a run's output,
+// which can be 1032 times the input it came from, for every buffer handed out.
+static void inflater_trim_output(InflaterH *d) {
+	const int64_t keep_from = d->delivered < d->rs_out ? d->delivered : d->rs_out;
+	if (keep_from > d->out_base) {
+		d->output.erase(d->output.begin(), d->output.begin() + (keep_from - d->out_base));
+		d->out_base = keep_from;
+	}
+}
+
+// decodes from the resume point to the end of what is available; appends to output, fills consumed / raw_done and moves
+// the resume point forward
+static int inflater_run_device(InflaterH *d) {
+	inflater_trim_output(d);
+	int64_t cap = 0;
 	for (int attempt = 0; attempt < 8; attempt++) {
-		const int64_t D = (int64_t)d->window.size();
+		// slot: window image, header copy, compressed bytes from the resume point's byte on
+		const int64_t tail_byte = d->rs_bit >> 3, slice_abs = d->raw_off + tail_byte;
+		const int64_t avail = d->in_total - slice_abs, H = (int64_t)d->hdr.size();
+		if (avail < 0 || slice_abs < d->in_base) {
+			set_error("inflater resume point outside the kept input");
+			return B200Z_E_INTERNAL;
+		}
+		const int64_t comp = H + avail, D = (int64_t)d->window.size();
+		const int32_t sbit = H ? d->hdr_sbit : (int32_t)(d->rs_bit & 7);
+		const int64_t skip = H ? 8 * H + (d->rs_bit & 7) : 0;
+		cap = std::max(cap, comp * 8 + 65536);
 		int rc;
-		if (!d->plan || avail > d->plan_comp_cap || cap > d->plan_out_cap) {
+		if (!d->plan || comp > d->plan_comp_cap || cap > d->plan_out_cap) {
 			b200z_plan_destroy(d->plan);
 			d->plan = nullptr;
 			int64_t cc = 65536;
-			while (cc < avail) cc *= 2;
+			while (cc < comp) cc *= 2;
 			const int64_t oc = std::max(cap, cc * 8 + 65536), dc = 32768;
 			if ((rc = b200z_inflate_plan_create_ex(1, &cc, &oc, B200Z_WRAP_RAW, &dc, &d->plan))) return rc;
 			d->plan_comp_cap = cc;
 			d->plan_out_cap = oc;
 		}
 		b200z_plan *plan = d->plan;
-		if ((rc = b200z_inflate_plan_set_lengths(plan, &avail, &D))) return rc;
-		if ((rc = b200z_inflate_plan_set_start_bits(plan, &sbit))) return rc;
-		const uint8_t *inp = d->input.data() + (slice_abs - d->in_base);
+		if ((rc = b200z_inflate_plan_set_lengths(plan, &comp, &D))) return rc;
+		if ((rc = b200z_inflate_plan_set_resume(plan, &sbit, &skip))) return rc;
 		std::vector<uint8_t> slot;
-		if (D) { // window image (dictionary, earlier output) directly in front of the compressed bytes
-			slot.reserve((size_t)(D + avail));
-			slot.insert(slot.end(), d->window.begin(), d->window.end());
-			slot.insert(slot.end(), inp, inp + avail);
-			inp = slot.data();
-		}
-		rc = handle_run(plan, d->st, inp, nullptr);
+		slot.reserve((size_t)(D + comp));
+		slot.insert(slot.end(), d->window.begin(), d->window.end());
+		slot.insert(slot.end(), d->hdr.begin(), d->hdr.end());
+		const uint8_t *inp = d->input.data() + (slice_abs - d->in_base);
+		slot.insert(slot.end(), inp, inp + avail);
+		rc = handle_run(plan, d->st, slot.data(), nullptr);
 		const PipeMeta &r = d->st.h;
-		int64_t rbit = 0, rout = 0;
-		if (!rc) rc = b200z_plan_get_restart_points(plan, &rbit, &rout, nullptr);
+		int64_t hb = 0, bb = 0, sb = 0, so = 0;
+		if (!rc) rc = b200z_plan_get_resume_points(plan, &hb, &bb, &sb, &so, nullptr);
 		if (rc) return rc;
 		const int st = r.status[0] & 0xFF, detail = (r.status[0] >> 8) & 0xFF;
-		if (st == B200Z_E_NOMEM) {
-			cap = d->plan_out_cap * 8; // (the next attempt makes a larger plan)
-			continue;
-		}
-		// this run's output is output[rs_out, rs_out + out_len): it replaces what an earlier run decoded behind the
-		// restart point (the same bytes, and at least as many)
+		const int64_t olen = r.out_len[0];
+		d->stats[0]++;
+		d->stats[1] += olen;
+		// this run's output is output[rs_out, rs_out + olen) (what it decoded in front of an error is delivered too)
 		const uint8_t *o = d->st.hout.p + plan->out_off[0];
 		d->output.resize((size_t)(d->rs_out - d->out_base));
-		d->output.insert(d->output.end(), o, o + r.out_len[0]);
-		if (st == B200Z_OK) {
-			d->finished = true;
-			d->consumed = slice_abs + r.in_used[0];
-		} else if (st == B200Z_E_NEED_INPUT) {
-			d->consumed = d->in_total;
-		} else {
+		d->output.insert(d->output.end(), o, o + olen);
+		if (st != B200Z_OK && st != B200Z_E_NEED_INPUT && st != B200Z_E_NOMEM) {
 			d->error = st;
 			d->error_msg = inflate_detail_msg(detail);
 			return B200Z_OK;
 		}
-		if (rout < 0 || rout > r.out_len[0] || rbit < sbit || rbit > 8 * avail) {
-			set_error("inflater restart point out of range");
+		if (st == B200Z_OK) {
+			d->raw_done = true;
+			d->trailer_at = slice_abs + r.in_used[0] - H; // (the final block ends behind the header copy)
+			d->consumed = d->trailer_at;
+			return inflater_advance(d, olen);
+		}
+		if (so < 0 || so > olen || hb > bb || bb > sb || sb > 8 * comp || (sb < 8 * H && so != 0)) {
+			set_error("inflater resume point out of range");
 			return B200Z_E_INTERNAL;
 		}
-		if (rout > 0 || rbit != sbit) {
-			// move the restart point: checksum and window advance over output[rs_out, rs_out + rout)
-			const uint8_t *seg = d->output.data() + (d->rs_out - d->out_base);
-			if (!d->raw && rout > 0 && (rc = b200z_adler32(seg, rout, &d->run_adler))) return rc;
-			if (rout >= 32768) d->window.assign(seg + rout - 32768, seg + rout);
-			else {
-				d->window.insert(d->window.end(), seg, seg + rout);
-				if (d->window.size() > 32768) d->window.erase(d->window.begin(), d->window.end() - 32768);
-			}
-			d->rs_out += rout;
-			d->rs_bit = (d->rs_bit & ~7ll) + rbit;
+		if (sb >= 8 * H) { // (in front of that only when a run stopped before its first symbol)
+			if ((rc = inflater_advance(d, so))) return rc;
+			const uint8_t *c = slot.data() + D;
+			if (bb != hb) d->hdr.assign(c + (hb >> 3), c + ((bb + 7) >> 3)); // inside a Huffman block: keep its header
+			else d->hdr.clear();
+			d->hdr_sbit = (int32_t)(hb & 7);
+			d->rs_bit = 8 * tail_byte + (sb - 8 * H);
 		}
-		if (st == B200Z_E_NEED_INPUT) {
-			// compressed bytes in front of the restart point are never looked at again
-			const int64_t keep_from = d->raw_off + (d->rs_bit >> 3);
-			if (keep_from > d->in_base) {
-				d->input.erase(d->input.begin(), d->input.begin() + (keep_from - d->in_base));
-				d->in_base = keep_from;
-			}
+		if (st == B200Z_E_NOMEM) {
+			cap = d->plan_out_cap * 8; // (the next attempt makes a larger plan and goes on from the resume point)
+			continue;
+		}
+		d->consumed = d->in_total;
+		// compressed bytes in front of the resume point are never looked at again
+		const int64_t keep_from = d->raw_off + (d->rs_bit >> 3);
+		if (keep_from > d->in_base) {
+			d->input.erase(d->input.begin(), d->input.begin() + (keep_from - d->in_base));
+			d->in_base = keep_from;
 		}
 		return B200Z_OK;
 	}
@@ -421,14 +459,6 @@ static int inflater_run_device(InflaterH *d) {
 	return B200Z_E_NOMEM;
 }
 
-// output in front of both the restart point and the delivery position is not needed any more
-static void inflater_trim_output(InflaterH *d) {
-	const int64_t keep_from = d->delivered < d->rs_out ? d->delivered : d->rs_out;
-	if (keep_from - d->out_base >= 65536) {
-		d->output.erase(d->output.begin(), d->output.begin() + (keep_from - d->out_base));
-		d->out_base = keep_from;
-	}
-}
 
 } // namespace b200z
 
@@ -677,10 +707,14 @@ int b200z_inflater_reset(void *h) {
 	d->input.clear();
 	d->output.clear();
 	d->window.clear();
-	d->new_input = d->finished = d->need_dict = d->header_done = false;
+	d->new_input = d->finished = d->need_dict = d->header_done = d->raw_done = false;
 	d->in_base = d->in_total = 0;
+	d->trailer_at = 0;
 	d->raw_off = 0;
 	d->rs_bit = d->rs_out = 0;
+	d->hdr.clear();
+	d->hdr_sbit = 0;
+	for (int64_t &v : d->stats) v = 0;
 	d->run_adler = 1;
 	d->out_base = 0;
 	d->delivered = 0;
@@ -735,6 +769,7 @@ int b200z_inflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 	d->input.insert(d->input.end(), buf, buf + len);
 	d->in_total += len;
 	d->new_input = true;
+	d->note_held();
 	return B200Z_OK;
 }
 
@@ -792,28 +827,28 @@ int b200z_inflater_inflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 			d->new_input = true;
 			return B200Z_OK;
 		}
-		int rc = inflater_run_device(d);
-		if (rc) return rc;
-		if (d->finished && !d->raw) {
-			// Adler32 trailer, read MSB first (DecodeChksum :397-418); until it is complete the reference withholds
-			// nothing that was already decoded but is not "finished"
-			if (d->in_total - d->consumed < 4) {
-				d->finished = false;
+		if (!d->raw_done) {
+			int rc = inflater_run_device(d);
+			d->note_held();
+			if (rc) return rc;
+		}
+		if (d->raw_done && d->raw) {
+			d->finished = true;
+		} else if (d->raw_done) {
+			// Adler32 trailer, read MSB first (DecodeChksum :397-418); until it is complete only its bytes are awaited, the
+			// decoded output is all there
+			if (d->in_total - d->trailer_at < 4) {
 				d->consumed = d->in_total;
-				// keep output; the last block is decoded again when the trailer arrives
 			} else {
-				const uint8_t *t = d->input.data() + (d->consumed - d->in_base);
+				const uint8_t *t = d->input.data() + (d->trailer_at - d->in_base);
 				const uint32_t want = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
-				uint32_t got = d->run_adler; // output[0, rs_out) is in it already
-				const int64_t rest = d->out_total() - d->rs_out;
-				int rc2 = rest > 0 ? b200z_adler32(d->output.data() + (d->rs_out - d->out_base), rest, &got) : B200Z_OK;
-				if (rc2) return rc2;
-				d->adler = got;
-				if (got != want) {
+				d->adler = d->run_adler; // of all the output
+				if (d->run_adler != want) {
 					d->error = B200Z_E_DATA;
 					d->error_msg = "Adler chksum doesn't match";
 				}
-				d->consumed += 4;
+				d->consumed = d->trailer_at + 4;
+				d->finished = true;
 			}
 		}
 	}
@@ -822,7 +857,6 @@ int b200z_inflater_inflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 	if (take) memcpy(out, d->output.data() + (d->delivered - d->out_base), take);
 	d->delivered += (int64_t)take;
 	*produced = (int32_t)take;
-	inflater_trim_output(d);
 	if (take == 0 && d->error) {
 		set_error("%s", d->error_msg.c_str());
 		return d->error;
@@ -861,6 +895,15 @@ int b200z_inflater_total_out(void *h, int64_t *v) {
 int b200z_inflater_adler(void *h, uint32_t *v) {
 	InflaterH *d = (InflaterH *)h;
 	*v = d->raw ? 0u : d->adler;
+	return B200Z_OK;
+}
+int b200z_inflater_get_stats(void *h, int64_t *v, int32_t cap) {
+	if (!h || cap < 0 || (cap > 0 && !v)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	const InflaterH *d = (const InflaterH *)h;
+	for (int32_t i = 0; i < cap && i < 4; i++) v[i] = d->stats[i];
 	return B200Z_OK;
 }
 

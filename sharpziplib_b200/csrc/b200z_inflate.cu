@@ -23,6 +23,7 @@
 // reference window holds (trap T13: the reference does not check distances).
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 
 #include <cuda_pipeline.h>
@@ -212,6 +213,22 @@ constexpr int kMList = 32;                       // back-references a lane may r
 
 enum { F_EOB = 1, F_ERR = 2, F_OVERRUN = 4, F_DEAD = 8 };
 
+// What a run reports per stream about where decoding can go on: the last block header reached and the output in front of
+// it (the restart point, b200z_plan_get_restart_points), then the resume point (b200z_plan_get_resume_points): where that
+// block's symbols start, the first symbol not decoded and the output in front of it.  The resume point lies inside the
+// block only when the stream stopped inside a Huffman block for want of input or output space; otherwise it is the
+// restart point.
+constexpr int kRestartWords = 5;
+__device__ __forceinline__ void put_restart(int64_t *r, int i, uint64_t hdr_bit, uint64_t hdr_out, uint64_t body_bit,
+                                            uint64_t sym_bit, uint64_t sym_out) {
+	int64_t *p = r + (int64_t)kRestartWords * i;
+	p[0] = (int64_t)hdr_bit;
+	p[1] = (int64_t)hdr_out;
+	p[2] = (int64_t)body_bit;
+	p[3] = (int64_t)sym_bit;
+	p[4] = (int64_t)sym_out;
+}
+
 // The round's input lives in shared memory, so a lane needs no bit buffer: the 32 bits that start at any bit position
 // are two words and a funnel shift away.  The decode state of a lane is just its bit position.
 __device__ __forceinline__ uint32_t peek32(const uint32_t *w, uint32_t pos) {
@@ -339,7 +356,7 @@ __global__ void __launch_bounds__(kInfThreads)
               const int64_t *__restrict__ in_len, const int64_t *__restrict__ out_off, const int64_t *__restrict__ out_cap,
               int nstreams, int64_t *__restrict__ out_len, int64_t *__restrict__ in_used, int32_t *__restrict__ status,
               const uint32_t *__restrict__ dict_len, const uint32_t *__restrict__ start_bit, const int32_t *__restrict__ pre,
-              int64_t *__restrict__ restart, const int32_t *__restrict__ only) {
+              int64_t *__restrict__ restart, const int32_t *__restrict__ only, const int64_t *__restrict__ skip_bit) {
 	extern __shared__ __align__(16) uint8_t smem_raw[];
 	InfBlockShared &S = *reinterpret_cast<InfBlockShared *>(smem_raw);
 	const int lane = threadIdx.x & 31;
@@ -352,8 +369,7 @@ __global__ void __launch_bounds__(kInfThreads)
 			status[stream] = pre[stream];
 			out_len[stream] = 0;
 			if (in_used) in_used[stream] = 0;
-			restart[2 * stream] = 0;
-			restart[2 * stream + 1] = 0;
+			put_restart(restart, stream, 0, 0, 0, 0, 0);
 		}
 		return;
 	}
@@ -395,9 +411,14 @@ __global__ void __launch_bounds__(kInfThreads)
 	bool last = false, in_block = false, a_done = false, pending_stored = false;
 	uint32_t stored_len = 0;
 	// restart point: bit position of the last block header reached and the output position there.  A caller that only
-	// has part of a stream (the Inflater handle between SetInput calls) decodes on from this header instead of from the
-	// start: everything the decoder carries across a block boundary is the window (the output) and the bit position.
+	// has part of a stream can decode on from this header instead of from the start: everything the decoder carries
+	// across a block boundary is the window (the output) and the bit position.  Inside a Huffman block it carries the
+	// block's code tables as well, which its header gives again (the resume point, put_restart).
 	uint64_t rs_bit = bitpos, rs_out = 0;
+	uint64_t body_bit = bitpos; // where the symbols of the block at rs_bit start (rs_bit: a stored block or an unfinished header)
+	// a stream entered in mid-block (b200z_inflate_plan_set_resume): its first header is a copy, decoding goes on at skip
+	const uint64_t skip = skip_bit ? (uint64_t)skip_bit[stream] : 0u;
+	bool first_hdr = true;
 	int tab = 0, static_in = -1; // static_in: which table buffer currently holds the static tables (-1 none)
 
 	for (uint32_t t = 0;; t++) {
@@ -437,7 +458,9 @@ __global__ void __launch_bounds__(kInfThreads)
 						if (!last) {
 							rs_bit = bitpos;
 							rs_out = opos;
+							body_bit = bitpos;
 						}
+						uint64_t hend = bitpos;
 						if (lane == 0) {
 							// re-seat the header reader at the true bit position
 							br.consumed = bitpos;
@@ -531,7 +554,15 @@ __global__ void __launch_bounds__(kInfThreads)
 							}
 							// an error diagnosed from bits past the end of the input is "needs more input", not corrupt data
 							if (st != B200Z_OK && br.overrun()) { st = B200Z_E_NEED_INPUT; detail = 0; }
+							hend = br.consumed;
+							// only a Huffman block can be entered in the middle, and not inside its own header
+							if (st == B200Z_OK && first_hdr && skip) {
+								if (btype == 0 || hend > skip) { st = B200Z_E_ARG; detail = 0; }
+								else br.consumed = skip;
+							}
 						}
+						first_hdr = false;
+						hend = __shfl_sync(0xffffffffu, (unsigned long long)hend, 0);
 						st = __shfl_sync(0xffffffffu, st, 0);
 						btype = __shfl_sync(0xffffffffu, btype, 0);
 						last = __shfl_sync(0xffffffffu, (int)last, 0) != 0;
@@ -546,6 +577,7 @@ __global__ void __launch_bounds__(kInfThreads)
 						} else {
 							tab = ntab;
 							in_block = true;
+							body_bit = hend;
 						}
 					}
 					if (in_block && !a_done) {
@@ -766,8 +798,9 @@ __global__ void __launch_bounds__(kInfThreads)
 			if (used > br.nbytes) used = br.nbytes;
 			in_used[stream] = (int64_t)used;
 		}
-		restart[2 * stream] = (int64_t)rs_bit;
-		restart[2 * stream + 1] = (int64_t)rs_out;
+		// (a round that did not fit the output leaves bitpos / opos at its first symbol, like one that ran out of input)
+		const bool mid = (st == B200Z_E_NEED_INPUT || st == B200Z_E_NOMEM) && body_bit != rs_bit;
+		put_restart(restart, stream, rs_bit, rs_out, mid ? body_bit : rs_bit, mid ? bitpos : rs_bit, mid ? opos : rs_out);
 	}
 }
 
@@ -887,17 +920,19 @@ namespace b200z {
 // ------------------------------------------------------------------------------------------------
 struct InflatePlan final : b200z_plan {
 	bool has_start_bits = false; // raw plans: caller-supplied first bit (b200z_inflate_plan_set_start_bits)
+	bool has_skip = false;       // raw plans: streams entered in mid-block (b200z_inflate_plan_set_resume)
 	std::vector<int64_t> comp_off, comp_cap, dict_cap; // where the compressed bytes start in the blob; capacities (b200z_inflate_plan_set_lengths)
 	// block-parallel pipeline (b200z_inflate_par.cuh)
 	bool inf_parallel = true; // false: the serial kernel only (B200Z_INFLATE=serial)
 	uint32_t nwin_total = 0, n_ftiles = 0, fs_cap = 0, round_cap = 0, hdr_cap = 0;
 	int dec1_grid = 0, dec2_grid = 0, find3_grid = 0;
 	int n_ck_tiles = 0;
-	// workspace: per stream the dictionary length, the first deflate bit and the framing's header verdict, and the (bit,
-	// output position) of the last block header reached; then the checksum scratch and the block-parallel pipeline's arrays
+	// workspace: per stream the dictionary length, the first deflate bit, the bit decoding jumps to behind a copied header and
+	// the framing's header verdict, and the restart and resume points (kRestartWords); then the checksum scratch and the
+	// block-parallel pipeline's arrays
 	Slot<uint32_t> o_hist, o_start_bit, o_win_base, o_win_stream, o_cand, o_seg_list, o_match_cap, o_str_nm;
 	Slot<int32_t> o_pre, o_fallback;
-	Slot<int64_t> o_restart, o_mt_off;
+	Slot<int64_t> o_restart, o_skip, o_mt_off;
 	Slot<unsigned long long> o_ck_acc, o_fs_list;
 	Slot<CkTile> o_ck_desc;
 	Slot<FTile> o_ftiles;
@@ -942,7 +977,8 @@ static int inflate_plan_build(InflatePlan *p) {
 	p->o_hist = ws.upload(dict32, 1);
 	p->o_start_bit = ws.reserve<uint32_t>(n + 1);
 	p->o_pre = ws.reserve<int32_t>(n + 1);
-	p->o_restart = ws.reserve<int64_t>(2ll * (n + 1));
+	p->o_restart = ws.reserve<int64_t>((int64_t)kRestartWords * (n + 1));
+	p->o_skip = ws.reserve<int64_t>(n + 1);
 	if (p->wrap != B200Z_WRAP_RAW) {
 		// checksum of the OUTPUT (Adler-32 for zlib, CRC-32 for gzip and raw+CRC): tiles over the capacities, the kernel takes
 		// the real lengths from d_out_len
@@ -1072,6 +1108,19 @@ int inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit) {
 	const int rc = p->ws.write(p->o_start_bit, std::vector<uint32_t>(start_bit, start_bit + p->n));
 	if (rc) return rc;
 	p->has_start_bits = true;
+	p->has_skip = false; // (a header, no jump: what an earlier set_resume asked for no longer holds)
+	return B200Z_OK;
+}
+
+int inflate_plan_set_resume(b200z_plan *plan, const int32_t *start_bit, const int64_t *skip_bit) {
+	InflatePlan *p = static_cast<InflatePlan *>(plan);
+	std::vector<uint32_t> sb((size_t)p->n);
+	for (int i = 0; i < p->n; i++) sb[(size_t)i] = (uint32_t)start_bit[i];
+	int rc = p->ws.write(p->o_start_bit, sb);
+	if (!rc) rc = p->ws.write(p->o_skip, std::vector<int64_t>(skip_bit, skip_bit + p->n));
+	if (rc) return rc;
+	p->has_start_bits = true;
+	p->has_skip = true;
 	return B200Z_OK;
 }
 
@@ -1098,16 +1147,28 @@ int inflate_plan_set_lengths(b200z_plan *plan, const int64_t *comp_len, const in
 	return rc ? rc : p->ws.write(p->o_hist, d32);
 }
 
-int inflate_plan_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_pos, cudaStream_t s) {
-	InflatePlan *p = static_cast<InflatePlan *>(plan);
-	std::vector<int64_t> rp(2 * (size_t)p->n);
-	B200Z_CUDA(cudaMemcpyAsync(rp.data(), p->ws.at(p->o_restart), 16ull * p->n, cudaMemcpyDeviceToHost, s));
+// the kRestartWords values per stream of the last run; `pick` lists which of them go to out[0], out[1], ...
+static int inflate_plan_read_points(InflatePlan *p, std::initializer_list<int> pick, int64_t *const *out, cudaStream_t s) {
+	std::vector<int64_t> rp((size_t)kRestartWords * p->n);
+	B200Z_CUDA(cudaMemcpyAsync(rp.data(), p->ws.at(p->o_restart), 8ull * rp.size(), cudaMemcpyDeviceToHost, s));
 	B200Z_CUDA(cudaStreamSynchronize(s));
-	for (int i = 0; i < p->n; i++) {
-		bit[i] = rp[2 * (size_t)i];
-		out_pos[i] = rp[2 * (size_t)i + 1];
+	int k = 0;
+	for (int w : pick) {
+		for (int i = 0; i < p->n; i++) out[k][i] = rp[(size_t)kRestartWords * i + (size_t)w];
+		++k;
 	}
 	return B200Z_OK;
+}
+
+int inflate_plan_restart_points(b200z_plan *plan, int64_t *bit, int64_t *out_pos, cudaStream_t s) {
+	int64_t *const out[2] = {bit, out_pos};
+	return inflate_plan_read_points(static_cast<InflatePlan *>(plan), {0, 1}, out, s);
+}
+
+int inflate_plan_resume_points(b200z_plan *plan, int64_t *hdr_bit, int64_t *body_bit, int64_t *sym_bit, int64_t *out_pos,
+                               cudaStream_t s) {
+	int64_t *const out[4] = {hdr_bit, body_bit, sym_bit, out_pos};
+	return inflate_plan_read_points(static_cast<InflatePlan *>(plan), {0, 2, 3, 4}, out, s);
 }
 
 int inflate_plan_stats(b200z_plan *plan, uint32_t *v, int32_t cap, cudaStream_t s) {
@@ -1147,6 +1208,7 @@ int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 	}
 	const int64_t *in_off = ws.at(p->o_in_off), *in_len = ws.at(p->o_in_len);
 	uint32_t *start_bit = (framed || p->has_start_bits) ? ws.at(p->o_start_bit) : nullptr;
+	const int64_t *skip_bit = p->has_skip ? ws.at(p->o_skip) : nullptr;
 	int32_t *pre = framed ? ws.at(p->o_pre) : nullptr;
 	if (framed) {
 		p->mark(s, "k_wrap");
@@ -1173,7 +1235,7 @@ int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 		B200Z_CUDA(cudaMemsetAsync(ctr, 0, sizeof(PCounters), s));
 		B200Z_CUDA(cudaMemsetAsync(cand, 0xFF, 4ull * p->nwin_total, s));
 		if (p->n_ftiles)
-			k_find<<<p->n_ftiles, 256, 0, s>>>(d_in, in_off, in_len, ws.at(p->o_ftiles), start_bit, pre, fs_list, ctr, p->fs_cap);
+			k_find<<<p->n_ftiles, 256, 0, s>>>(d_in, in_off, in_len, ws.at(p->o_ftiles), start_bit, skip_bit, pre, fs_list, ctr, p->fs_cap);
 		p->mark(s, "k_find3");
 		k_find3<<<p->find3_grid, 128, 0, s>>>(d_in, in_off, in_len, fs_list, ctr, p->fs_cap, win_base, cand);
 		p->mark(s, "k_seglist");
@@ -1182,7 +1244,7 @@ int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 		                                            seg_list, ctr);
 		p->mark(s, "k_dec1");
 		k_dec1<<<p->dec1_grid, kP1Threads, sizeof(Dec1Shared), s>>>(d_in, in_off, in_len, segs, seg_list, ctr, win_base, cand, rounds,
-		                                                             p->round_cap, hdrs, p->hdr_cap);
+		                                                             p->round_cap, hdrs, p->hdr_cap, skip_bit);
 		p->mark(s, "k_chain");
 		k_chain<<<(n + 127) / 128, 128, 0, s>>>(n, segs, win_base, in_len, out_cap, ws.at(p->o_match_cap), pre, d_out_len, d_in_used,
 		                                        d_status, restart, str_nm, fallback);
@@ -1195,7 +1257,7 @@ int inflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 	}
 	p->mark(s, "k_inflate");
 	k_inflate<<<n, kInfThreads, kInfSmem2, s>>>(d_in, d_out, in_off, in_len, out_off, out_cap, n, d_out_len, d_in_used, d_status, dict_len,
-	                                           start_bit, pre, restart, only);
+	                                           start_bit, pre, restart, only, skip_bit);
 	if (wrap != B200Z_WRAP_RAW) {
 		p->mark(s, "checksum");
 		int rc = checksum_launch(wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_out, out_off, d_out_len, n, ws.at(p->o_ck_desc), p->n_ck_tiles,

@@ -18,7 +18,7 @@
 //                      prefix sums of the bytes and back-references the lanes produce.
 //   k_chain            one thread per stream follows the segments from the stream start (join -> the candidate's segment
 //                      -> ...), gives every segment on the chain its output position, and derives what Inflater reports:
-//                      status, TotalOut, RemainingInput (trap T14), the restart point.
+//                      status, TotalOut, RemainingInput (trap T14), the restart and resume points.
 //   k_dec2             one CTA per recorded batch of rounds: the final decode pass, every lane from its recorded entry with
 //                      its recorded output position -- literals straight into the output buffer, back-references as
 //                      (position, length, distance) records in stream order.
@@ -55,6 +55,7 @@ struct FTile { // k_find: 2048 words of one stream
 
 struct __align__(16) PSeg {
 	uint64_t start_bit, end_bit, rs_bit;
+	uint64_t body_bit;          // where the symbols of the block at rs_bit start (rs_bit: a stored block or an unfinished header)
 	uint64_t out_bytes, rs_out; // relative to the segment's first output byte
 	uint64_t out_base;          // k_chain: output position of the segment
 	uint32_t stream, n_match, match_base;
@@ -98,8 +99,8 @@ __device__ __forceinline__ uint32_t ld_stream_word(const uint32_t *gwords, uint3
 // code-length code (a complete code: sum of 2^(7-len) = 128) through a table of four lengths at a time.
 __global__ void __launch_bounds__(256)
     k_find(const uint8_t *__restrict__ in, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len,
-           const FTile *__restrict__ tiles, const uint32_t *__restrict__ start_bit, const int32_t *__restrict__ pre,
-           unsigned long long *__restrict__ fs_list, PCounters *__restrict__ ctr, uint32_t fs_cap) {
+           const FTile *__restrict__ tiles, const uint32_t *__restrict__ start_bit, const int64_t *__restrict__ skip_bit,
+           const int32_t *__restrict__ pre, unsigned long long *__restrict__ fs_list, PCounters *__restrict__ ctr, uint32_t fs_cap) {
 	__shared__ uint8_t lut[4096];
 	__shared__ uint32_t sw[kFindTileWords + 4];
 	__shared__ uint16_t queue[8][1024];
@@ -117,7 +118,10 @@ __global__ void __launch_bounds__(256)
 	const uint32_t *gwords = reinterpret_cast<const uint32_t *>(in + in_off[t.stream]);
 	const uint32_t nbytes = (uint32_t)in_len[t.stream];
 	const uint32_t nwords = (nbytes + 3) >> 2;
-	const uint64_t sb = start_bit ? start_bit[t.stream] : 0u;
+	uint64_t sb = start_bit ? start_bit[t.stream] : 0u;
+	// a stream entered in mid-block (b200z_inflate_plan_set_resume): its chain jumps from the header copy to skip_bit, so
+	// nothing in front of that is a block it could join
+	if (skip_bit && (uint64_t)skip_bit[t.stream] > sb) sb = (uint64_t)skip_bit[t.stream];
 	const uint64_t total_bits = 8ull * nbytes;
 	for (uint32_t i = threadIdx.x; i < t.nwords + 4; i += 256) sw[i] = ld_stream_word(gwords, t.word0 + i, nwords, nbytes);
 	__syncthreads();
@@ -553,6 +557,7 @@ struct __align__(16) Dec1Shared {
 	// header results (thread 0 -> all)
 	int h_st, h_detail, h_btype, h_last, h_nlit, h_ndist;
 	unsigned long long h_bitpos;
+	unsigned long long h_body; // thread 0 only: where the current block's symbols start (its header bit if it has none)
 	uint32_t h_stored_len;
 	uint32_t q_idx, a_base;
 	int stop[2], front[2];
@@ -568,7 +573,7 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
     k_dec1(const uint8_t *__restrict__ in, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len, PSeg *__restrict__ segs,
            const uint32_t *__restrict__ seg_list, PCounters *__restrict__ ctr, const uint32_t *__restrict__ win_base,
            const uint32_t *__restrict__ cand, PRound *__restrict__ rounds, uint32_t round_cap, PBlockHdr *__restrict__ hdrs,
-           uint32_t hdr_cap) {
+           uint32_t hdr_cap, const int64_t *__restrict__ skip_bit) {
 	extern __shared__ __align__(16) uint8_t smem_raw[];
 	Dec1Shared &S = *reinterpret_cast<Dec1Shared *>(smem_raw);
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -684,6 +689,15 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
 				}
 				// an error diagnosed from bits past the end of the input is "needs more input", not corrupt data
 				if (hst != B200Z_OK && br.overrun()) { hst = B200Z_E_NEED_INPUT; hdet = 0; }
+				const uint64_t hend = br.consumed;
+				S.h_body = (hst == B200Z_OK && (btype == 1 || btype == 2)) ? hend : bitpos;
+				// the stream-start segment (slot == stream) of a stream entered in mid-block: the header is a copy, decoding goes on at
+				// skip_bit; only a Huffman block can be entered there, and not inside its own header
+				if (hst == B200Z_OK && !blocks_done && slot == stream && skip_bit && skip_bit[stream]) {
+					const uint64_t skip = (uint64_t)skip_bit[stream];
+					if (btype == 0 || hend > skip) { hst = B200Z_E_ARG; hdet = 0; }
+					else br.consumed = skip;
+				}
 				S.h_st = hst;
 				S.h_detail = hdet;
 				S.h_btype = btype;
@@ -931,6 +945,7 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
 		if (tid == 0) {
 			seg.end_bit = bitpos;
 			seg.rs_bit = rs_bit;
+			seg.body_bit = S.h_body;
 			seg.rs_out = rs_out;
 			seg.out_bytes = opos;
 			seg.n_match = nm_total;
@@ -955,21 +970,21 @@ __global__ void k_chain(int n, PSeg *__restrict__ segs, const uint32_t *__restri
 		status[i] = pre[i];
 		out_len[i] = 0;
 		if (in_used) in_used[i] = 0;
-		restart[2 * i] = 0;
-		restart[2 * i + 1] = 0;
+		put_restart(restart, i, 0, 0, 0, 0, 0);
 		return;
 	}
 	const uint32_t wb = win_base[i];
 	uint64_t out = 0, nm = 0;
 	uint32_t cur = (uint32_t)i;
 	int st = B200Z_OK;
-	uint64_t end_bit = 0, rs_bit = 0, rs_out = 0;
+	uint64_t end_bit = 0, rs_bit = 0, rs_out = 0, body_bit = 0;
 	bool pool = false;
 	// pass 1: totals
 	for (;;) {
 		const PSeg &s = segs[cur];
 		rs_bit = s.rs_bit;
 		rs_out = out + s.rs_out;
+		body_bit = s.body_bit;
 		out += s.out_bytes;
 		nm += s.n_match;
 		end_bit = s.end_bit;
@@ -990,8 +1005,8 @@ __global__ void k_chain(int n, PSeg *__restrict__ segs, const uint32_t *__restri
 		status[i] = B200Z_E_NOMEM;
 		out_len[i] = 0;
 		if (in_used) in_used[i] = 0;
-		restart[2 * i] = (int64_t)segs[i].start_bit;
-		restart[2 * i + 1] = 0;
+		const uint64_t sb = segs[i].start_bit;
+		put_restart(restart, i, sb, 0, sb, sb, 0);
 		return;
 	}
 	// pass 2: positions
@@ -1016,8 +1031,8 @@ __global__ void k_chain(int n, PSeg *__restrict__ segs, const uint32_t *__restri
 		if (used > (uint64_t)in_len[i]) used = (uint64_t)in_len[i];
 		in_used[i] = (int64_t)used;
 	}
-	restart[2 * i] = (int64_t)rs_bit;
-	restart[2 * i + 1] = (int64_t)rs_out;
+	const bool mid = (st & 0xFF) == B200Z_E_NEED_INPUT && body_bit != rs_bit; // the input ended inside a Huffman block
+	put_restart(restart, i, rs_bit, rs_out, mid ? body_bit : rs_bit, mid ? end_bit : rs_bit, mid ? out : rs_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------

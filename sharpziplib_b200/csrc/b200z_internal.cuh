@@ -206,6 +206,9 @@ int inflate_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_c
 int inflate_plan_set_start_bits(b200z_plan *p, const int32_t *start_bit);
 int inflate_plan_set_lengths(b200z_plan *p, const int64_t *comp_len, const int64_t *dict_len);
 int inflate_plan_restart_points(b200z_plan *p, int64_t *bit, int64_t *out_pos, cudaStream_t s);
+int inflate_plan_set_resume(b200z_plan *p, const int32_t *start_bit, const int64_t *skip_bit);
+int inflate_plan_resume_points(b200z_plan *p, int64_t *hdr_bit, int64_t *body_bit, int64_t *sym_bit, int64_t *out_pos,
+                               cudaStream_t s);
 int inflate_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s);
 int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_in_used, cudaStream_t s);
