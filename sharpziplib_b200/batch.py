@@ -87,77 +87,48 @@ class DeflatePlan(_Plan):
         history and chunk_lens may then come together.  undrained: per stream, Flush() / Finish() follows the last SetInput
         without a Deflate() call in between."""
         lens = np.ascontiguousarray(in_lens, dtype=np.int64)
-        h = C.c_void_p()
-        if state is not None:
-            self._fast_state(lens, level, strategy, wrap, end_mode, dict_lens, chunk_lens, history, state, undrained, h)
-        elif history is not None:
-            hl = np.ascontiguousarray(history[0], dtype=np.int64)
-            pb = np.ascontiguousarray(history[1], dtype=np.int64)
-            bb = np.ascontiguousarray(history[2], dtype=np.int32)
-            assert hl.size == lens.size and pb.size == lens.size and bb.size == lens.size
-            masks = [np.zeros(max(int(x), 1), np.uint8) for x in hl]
-            if len(history) > 3:
-                masks = [np.ascontiguousarray(np.frombuffer(bytes(m) + b"\0", np.uint8)) for m in history[3]]
-            mptrs = (C.c_void_p * lens.size)(*[m.ctypes.data for m in masks])
-            hs = _lib.History(_lib.HIST_CONTINUE, 0, hl.ctypes.data, pb.ctypes.data, bb.ctypes.data, C.addressof(mptrs))
-            _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(lens.size, lens.ctypes.data, level, strategy, wrap, end_mode,
-                                                                  C.addressof(hs), C.byref(h)))
-            self.dict_lens = hl
-        elif chunk_lens is not None:
-            assert len(chunk_lens) == lens.size
-            arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in chunk_lens]
-            counts = np.array([a.size for a in arrs], dtype=np.int32)
-            ptrs = (C.c_void_p * lens.size)(*[a.ctypes.data if a.size else None for a in arrs])
-            dl = None if dict_lens is None else np.ascontiguousarray(dict_lens, dtype=np.int64)
-            hs = _lib.History(_lib.HIST_NONE if dl is None else _lib.HIST_DICTIONARY, 0, None if dl is None else dl.ctypes.data,
-                              None, None, None, counts.ctypes.data, C.addressof(ptrs), None, None, None)
-            _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(lens.size, lens.ctypes.data, level, strategy, wrap, end_mode,
-                                                                  C.addressof(hs), C.byref(h)))
-            self.dict_lens = np.zeros(lens.size, dtype=np.int64) if dl is None else dl
-        elif dict_lens is None:
-            _lib.raise_for(_lib.lib().b200z_deflate_plan_create(lens.size, lens.ctypes.data, level, strategy, wrap, end_mode,
-                                                               C.byref(h)))
-            self.dict_lens = np.zeros(lens.size, dtype=np.int64)
-        else:
-            dl = np.ascontiguousarray(dict_lens, dtype=np.int64)
-            hs = _lib.History(_lib.HIST_DICTIONARY, 0, dl.ctypes.data, None, None, None)
-            _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(lens.size, lens.ctypes.data, level, strategy, wrap, end_mode,
-                                                                  C.addressof(hs), C.byref(h)))
-            self.dict_lens = dl
-        self.in_lens = lens
-        self.level = level
-        super().__init__(h, lens.size)
-        if entry is not None:
-            self.set_entry(entry)
-
-    def _fast_state(self, lens, level, strategy, wrap, end_mode, dict_lens, chunk_lens, history, state, undrained, h):
         n = lens.size
+        kind, hl, pb, bb, masks = _lib.HIST_NONE, None, None, None, None
         if history is not None:
-            kind, hl = _lib.HIST_CONTINUE, np.ascontiguousarray(history[0], dtype=np.int64)
-            pb = np.ascontiguousarray(history[1], dtype=np.int64)
+            kind, hl, pb = _lib.HIST_CONTINUE, np.ascontiguousarray(history[0], np.int64), np.ascontiguousarray(history[1], np.int64)
             bb = np.ascontiguousarray(history[2], dtype=np.int32)
-        else:
-            kind = _lib.HIST_NONE if dict_lens is None else _lib.HIST_DICTIONARY
-            hl = np.zeros(n, np.int64) if dict_lens is None else np.ascontiguousarray(dict_lens, dtype=np.int64)
-            pb = bb = None
-        cl = chunk_lens if chunk_lens is not None else [[int(x)] for x in lens]
-        arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in cl]
-        counts = np.array([a.size for a in arrs], dtype=np.int32)
-        ptrs = (C.c_void_p * n)(*[a.ctypes.data if a.size else None for a in arrs])
-        und = np.ascontiguousarray(undrained if undrained is not None else np.zeros(n), dtype=np.int32)
-        if level == 0:
+            assert hl.size == n and pb.size == n and bb.size == n
+            marr = None  # (with a state and no masks the library flags the last two history positions)
+            if len(history) > 3:
+                marr = [np.frombuffer(bytes(m) + b"\0", np.uint8) for m in history[3]]
+            elif state is None:  # nothing flagged: what a cut leaves
+                marr = [np.zeros(max(int(x), 1), np.uint8) for x in hl]
+            masks = None if marr is None else _ptr_array(marr)
+        elif dict_lens is not None:
+            kind, hl = _lib.HIST_DICTIONARY, np.ascontiguousarray(dict_lens, dtype=np.int64)
+        if chunk_lens is None and state is not None:
+            chunk_lens = [[int(x)] for x in lens]  # one SetInput with everything
+        counts = chunks = und = eng = st = None
+        if chunk_lens is not None:
+            assert len(chunk_lens) == n
+            arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in chunk_lens]
+            counts, chunks = np.array([a.size for a in arrs], dtype=np.int32), _ptr_array(arrs)
+        if undrained is not None:
+            und = np.ascontiguousarray(undrained, dtype=np.int32)
+        if state is not None and level == 0:
             assert isinstance(state, np.ndarray) and state.dtype == np.uint8 and state.size == 16 * n
-            eng, st = None, state.ctypes.data
-        else:
+            st = state.ctypes.data
+        elif state is not None:
             assert len(state) == n
-            eng, st = (C.c_void_p * n)(*[t.data_ptr() for t in state]), None
-        hs = _lib.History(kind, 0, hl.ctypes.data, None if pb is None else pb.ctypes.data, None if bb is None else bb.ctypes.data,
-                          None, counts.ctypes.data, C.addressof(ptrs), und.ctypes.data,
-                          None if eng is None else C.addressof(eng), st)
+            eng = (C.c_void_p * n)(*[t.data_ptr() for t in state])
+        self._state = state  # (levels 0-4: the plan and its runs write it)
+        addr = lambda a: None if a is None else a.ctypes.data  # noqa: E731
+        ref = lambda a: None if a is None else C.addressof(a)  # noqa: E731
+        hs = _lib.History(kind, 0, addr(hl), addr(pb), addr(bb), ref(masks), addr(counts), ref(chunks), addr(und), ref(eng), st)
+        h = C.c_void_p()
         _lib.raise_for(_lib.lib().b200z_deflate_plan_create_ex(n, lens.ctypes.data, level, strategy, wrap, end_mode,
                                                               C.addressof(hs), C.byref(h)))
-        self.dict_lens = hl
-        self._state = state  # (levels 1-4: the runs write it)
+        self.dict_lens = np.zeros(n, dtype=np.int64) if hl is None else hl
+        self.in_lens = lens
+        self.level = level
+        super().__init__(h, n)
+        if entry is not None:
+            self.set_entry(entry)
 
     def set_entry(self, entry):
         """per stream (prev_available, match_len, match_dist): the parse state the next runs start from"""

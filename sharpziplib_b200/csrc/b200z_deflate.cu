@@ -1594,70 +1594,99 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
+// A plan runs one of three engines, chosen by its level: the lazy parse (5-9), DeflateFast (1-4, k_fast) or DeflateStored
+// (0, k_stored).  Each engine has its own part of the plan, laid out by its *_layout function and launched by its *_launch
+// function; deflate_plan_build and deflate_plan_run do what is common and pick the engine.
 struct DeflatePlan final : b200z_plan {
-	// with history (b200z_deflate_plan_create_ex)
+	// common, per stream (b200z_deflate_plan_create_ex): the history in front of the data, the bits in front of the output
 	int hist_kind = 0; // B200Z_HIST_*
 	bool check_seeded = false;
-	std::vector<int64_t> pos_base;
-	std::vector<int32_t> bit_base;
-	std::vector<std::vector<uint8_t>> hist_mask;
-	// levels 0-4: the SetInput schedule of every stream (cumulative sizes), "Flush()/Finish() behind an undrained SetInput",
-	// and the engine state carried between the segments of a stream (b200z_history)
-	std::vector<std::vector<uint32_t>> sched_cum;
+	std::vector<int64_t> bias;     // stream position of the slot's first byte (pos_base - history)
+	std::vector<uint32_t> bit_base;
+	// levels 0-4: the SetInput schedule (cumulative sizes of stream i's calls at sched[sched_off[i] .. sched_off[i + 1]]),
+	// and "Flush()/Finish() behind an undrained SetInput"
+	std::vector<uint32_t> sched, sched_off;
 	std::vector<int32_t> undrained;
-	std::vector<void *> engine_state;           // device pointers (levels 1-4)
-	b200z_stored_state *stored_state = nullptr; // caller's host array (level 0), used while the plan is built
-	int n_runs = 0, n_tiles = 0, n_blkmax = 0, n_chunks = 0, n_rgroups = 0, n_stored = 0, n_ck_tiles = 0;
-	uint32_t parse_chunk = 32768;
-	int link_run = 65536; // positions per k_links CTA (B200Z_LINK_RUN)
-	int fast_prev_entries = 32768; // k_fast's prev[] size for this batch
-	int fast_ctas = 1;             // k_fast's persistent CTAs (each owns a head[] slot of the pool)
-	bool fast_head_smem = false;   // ... or keeps head[] in shared memory (few streams)
-	// workspace (deflate_plan_build lays it out)
-	Slot<uint32_t> o_blk_off, o_nsyms, o_nblocks, o_blk_start, o_blk_ptop, o_sym, o_hist, o_bitbase;
-	Slot<int64_t> o_bias, o_hm_off, o_ck_off, o_ck_len;
-	Slot<int2> o_run_desc, o_tile_desc, o_rgroups;
+	bool cut_ready = false; // an open run has been launched since the plan was made
+	int n_ck_tiles = 0;
+	Slot<uint32_t> o_hist, o_bitbase;
+	Slot<int64_t> o_bias, o_ck_off, o_ck_len;
+	Slot<CkTile> o_ck_desc;
+	Slot<unsigned long long> o_ck_acc;
+	// levels 1-9: the symbols and the blocks they are cut into (blocks_layout)
+	int n_blkmax = 0;
+	Slot<uint32_t> o_sym, o_blk_off, o_nsyms, o_nblocks, o_blk_start, o_blk_ptop;
 	Slot<int32_t> o_blk_desc;
 	Slot<BlockMeta> o_meta;
 	Slot<BlockTables> o_tables;
-	Slot<uint8_t> o_hmask;
-	Slot<CkTile> o_ck_desc;
-	Slot<unsigned long long> o_ck_acc;
-	Slot<uint16_t> o_link; // levels 5-9
-	Slot<uint2> o_mt;
-	Slot<uint32_t> o_sym_local, o_rnd_off, o_rnd_symoff;
-	Slot<ChunkDesc> o_chunks;
-	Slot<RoundRec> o_recs, o_ents;
-	Slot<RoundRec> o_entry, o_cut; // per stream: the parse state a run starts from, and where an open run stopped
-	std::vector<RoundRec> entry;   // what o_entry holds (b200z_deflate_plan_set_entry; a clean start by default)
-	bool cut_ready = false;        // an open run has been launched since the plan was made
-	Slot<StoredBlock> o_stored; // level 0
-	Slot<int64_t> o_slens;
-	Slot<uint32_t> o_sched, o_sched_off, o_fcounter; // levels 1-4
-	Slot<int32_t> o_undrained;
-	Slot<uint8_t *> o_fstate;
-	Slot<uint16_t> o_fhead;
-	Slot<uint2> o_fcut; // levels 1-4, open runs: per stream (covered, SetInput call) of the last cut, (0, 0) for none
-	std::vector<uint2> stored_cut; // level 0, open runs: the same, known when the plan is built
+	struct { // levels 5-9 (lazy_layout)
+		int link_run = 65536; // positions per k_links CTA (B200Z_LINK_RUN)
+		uint32_t parse_chunk = 32768;
+		int n_runs = 0, n_tiles = 0, n_chunks = 0, n_rgroups = 0;
+		std::vector<std::vector<uint8_t>> hist_mask; // (b200z_history.hist_mask; empty: the default)
+		Slot<int2> o_run_desc, o_tile_desc, o_rgroups;
+		Slot<int64_t> o_hm_off;
+		Slot<uint8_t> o_hmask;
+		Slot<uint16_t> o_link;
+		Slot<uint2> o_mt;
+		Slot<uint32_t> o_sym_local, o_rnd_off, o_rnd_symoff;
+		Slot<ChunkDesc> o_chunks;
+		Slot<RoundRec> o_recs, o_ents;
+		Slot<RoundRec> o_entry, o_cut; // per stream: the parse state a run starts from, and where an open run stopped
+		std::vector<RoundRec> entry;   // what o_entry holds (b200z_deflate_plan_set_entry; a clean start by default)
+	} lazy;
+	struct { // levels 1-4 (fast_layout)
+		std::vector<uint8_t *> engine_state; // per stream, the engine state carried between its segments (device pointers)
+		int prev_entries = 32768;         // k_fast's prev[] size for this batch
+		int ctas = 1;                     // k_fast's persistent CTAs (each owns a head[] slot of the pool)
+		bool head_smem = false;           // ... or keeps head[] in shared memory (few streams)
+		Slot<uint32_t> o_sched, o_sched_off, o_counter;
+		Slot<int32_t> o_undrained;
+		Slot<uint8_t *> o_state;
+		Slot<uint16_t> o_head;
+		Slot<uint2> o_cut; // open runs: per stream (covered, SetInput call) of the last cut, (0, 0) for none
+	} fast;
+	struct { // level 0 (stored_layout)
+		b200z_stored_state *state = nullptr; // caller's host array, used while the plan is built
+		int n_blocks = 0;
+		Slot<StoredBlock> o_blocks;
+		Slot<int64_t> o_lens;
+		std::vector<uint2> cut; // open runs: the same as fast.o_cut, known when the plan is built
+	} stored;
 };
 
-static int deflate_plan_build(DeflatePlan *p) {
-	const LevelParams lp = level_params(p->level);
+static int64_t hist_len(const DeflatePlan *p, int i) { return p->hist.empty() ? 0 : p->hist[i]; }
+
+// levels 1-9: room for each stream's symbols and for the most blocks they can be cut into
+static void blocks_layout(DeflatePlan *p) {
 	const int n = p->n;
-	std::vector<StoredBlock> sblocks; // level 0 only
-	std::vector<int64_t> slens;
-	p->in_off.resize(n);
-	p->out_off.resize(n);
-	p->out_cap.resize(n);
-	int64_t io = 0, oo = 0;
-	std::vector<int2> runs, tiles, rgroups;
-	std::vector<ChunkDesc> chunks;
-	std::vector<uint32_t> rnd_off(n + 1);
-	uint32_t nrounds = 0;
-	int64_t maxlen = 0;
-	for (int i = 0; i < n; i++) maxlen = p->in_len[i] > maxlen ? p->in_len[i] : maxlen;
-	int sms = 0;
-	if (sm_count(&sms) != cudaSuccess) sms = 132;
+	std::vector<uint32_t> blk_off(n + 1);
+	std::vector<int32_t> blk_desc;
+	uint32_t nblk = 0;
+	for (int i = 0; i < n; i++) {
+		blk_off[i] = nblk;
+		const uint32_t maxb = (uint32_t)(p->in_len[i] / kBlockSyms) + 2;
+		blk_desc.insert(blk_desc.end(), maxb, i);
+		nblk += maxb;
+	}
+	blk_off[n] = nblk;
+	p->n_blkmax = (int)nblk;
+	Arena &ws = p->ws;
+	p->o_sym = ws.reserve<uint32_t>(p->in_bytes + 16);
+	p->o_blk_desc = ws.upload(blk_desc, 1);
+	p->o_blk_off = ws.upload(blk_off);
+	p->o_nsyms = ws.reserve<uint32_t>(n);
+	p->o_nblocks = ws.reserve<uint32_t>(n);
+	p->o_blk_start = ws.reserve<uint32_t>(nblk + 1);
+	p->o_blk_ptop = ws.reserve<uint32_t>(nblk + 1);
+	p->o_meta = ws.reserve<BlockMeta>(nblk + 1);
+	p->o_tables = ws.reserve<BlockTables>(nblk + 1);
+}
+
+// levels 5-9
+static void lazy_layout(DeflatePlan *p, int64_t maxlen, int sms) {
+	auto &z = p->lazy;
+	const int n = p->n;
 	// chunk of the parse: 32 Ki positions (one warp each); k_parse_fix only compares states at their boundaries, so a long
 	// stream may have tens of thousands of them (grown beyond 65536 chunks per stream)
 	uint32_t chunk = 32768;
@@ -1665,11 +1694,12 @@ static int deflate_plan_build(DeflatePlan *p) {
 		const int64_t need = (maxlen / 65536 + kRound - 1) / kRound * kRound;
 		if (need > (int64_t)chunk) chunk = (uint32_t)need;
 	}
+	z.parse_chunk = chunk;
 	// Run length of k_links (a multiple of 32768, 65536 .. 1048576).  Every run but a stream's first re-walks 32768 positions
 	// to warm its head table up (37 % more steps than positions with 64 Ki runs on 256 KiB buffers, 12 % with 128 Ki runs,
 	// none with 256 Ki runs), while fewer, longer CTAs fill the last wave worse (three CTAs fit an SM).  The plan takes the
 	// length with the smallest estimate of waves x steps per run; B200Z_LINK_RUN=<positions> overrides it for timing.
-	p->link_run = kRun;
+	z.link_run = kRun;
 	{
 		const int64_t slots = 3ll * sms;
 		double best = 0;
@@ -1685,62 +1715,25 @@ static int deflate_plan_build(DeflatePlan *p) {
 			const double est = (double)((ctas + slots - 1) / slots) * (double)longest;
 			if (best == 0 || est < best * 0.97) { // (a longer run has to win clearly: its CTAs are the less balanced ones)
 				best = est;
-				p->link_run = (int)run;
+				z.link_run = (int)run;
 			}
 			if (run >= maxlen) break;
 		}
 	}
 	if (const char *e = getenv("B200Z_LINK_RUN")) {
 		const long v = atol(e);
-		if (v >= 65536 && v <= 1048576 && v % 32768 == 0) p->link_run = (int)v;
+		if (v >= 65536 && v <= 1048576 && v % 32768 == 0) z.link_run = (int)v;
 	}
-	p->parse_chunk = chunk;
-	{
-		// levels 1-4: size of k_fast's prev[] table (see there)
-		int64_t need = maxlen + 2;
-		int pe = 32768;
-		if (need <= 32768 && p->engine_state.empty()) pe = (int)((need + 255) / 256 * 256); // (a carried state holds whole tables)
-		p->fast_prev_entries = pe;
-		// persistent one-warp CTAs: as many per SM as their prev[] tables fit (head[] is in the pool), 16 at most
-		int per_sm = (int)((227 * 1024) / (2 * pe + 1024));
-		if (per_sm > 16) per_sm = 16;
-		if (per_sm < 1) per_sm = 1;
-		const int64_t slots = (int64_t)sms * per_sm;
-		p->fast_ctas = (int)(n < slots ? n : slots);
-		p->fast_head_smem = n <= sms; // nothing to gain from sharing SMs: keep head[] next to prev[] (k_fast)
-		if (const char *e = getenv("B200Z_FAST_HEAD")) p->fast_head_smem = e[0] == 's'; // "smem" / "pool": for tests and timing
-	}
-	std::vector<uint32_t> blk_off(n + 1);
-	std::vector<int32_t> blk_desc;
-	uint32_t nblk = 0;
-	const bool has_hist = !p->hist.empty();
-	std::vector<uint32_t> hist32(n, 0u), bitbase32(n, 0u);
-	std::vector<int64_t> bias64(n, 0), hm_off(n, 0);
+	std::vector<int2> runs, tiles, rgroups;
+	std::vector<ChunkDesc> chunks;
+	std::vector<uint32_t> rnd_off(n + 1);
+	std::vector<int64_t> hm_off(n, 0);
 	std::vector<uint8_t> hmask;
-	std::vector<int64_t> stored_taken(n, -1);
+	uint32_t nrounds = 0;
+	z.entry.resize(n);
 	for (int i = 0; i < n; i++) {
-		const int64_t len = p->in_len[i];
-		if (len < 0 || len > 0xFFFF0000ll) {
-			set_error("stream %d: length %lld out of range", i, (long long)len);
-			return B200Z_E_ARG;
-		}
-		const int64_t H = has_hist ? p->hist[i] : 0;
-		if (has_hist) {
-			hist32[i] = (uint32_t)H;
-			bias64[i] = p->pos_base[i] - H;
-			bitbase32[i] = (uint32_t)p->bit_base[i];
-			hm_off[i] = (int64_t)hmask.size();
-			hmask.resize(hmask.size() + (size_t)H + 1, 0);
-			uint8_t *m = hmask.data() + hm_off[i];
-			if (i < (int)p->hist_mask.size() && !p->hist_mask[i].empty()) memcpy(m, p->hist_mask[i].data(), (size_t)H);
-			else if (H) m[H - 1] = 1, m[H > 1 ? H - 2 : 0] = 1; // the last two positions of a dictionary/segment are never inserted
-		}
-		p->in_off[i] = io;
-		io += align_up(len + 16, kAlign);
-		p->out_off[i] = oo;
-		p->out_cap[i] = align_up(b200z_deflate_bound(len), kAlign);
-		oo += p->out_cap[i];
-		for (int64_t s = 0; s < len; s += p->link_run) runs.push_back(make_int2(i, (int)s));
+		const int64_t len = p->in_len[i], H = hist_len(p, i);
+		for (int64_t s = 0; s < len; s += z.link_run) runs.push_back(make_int2(i, (int)s));
 		for (int64_t s = 0; s < len; s += kTile) tiles.push_back(make_int2(i, (int)s));
 		for (int64_t s = 0; s < len; s += chunk)
 			chunks.push_back(ChunkDesc{i, (uint32_t)s, (uint32_t)(len - s > (int64_t)chunk ? s + chunk : len)});
@@ -1748,127 +1741,223 @@ static int deflate_plan_build(DeflatePlan *p) {
 		const uint32_t nr = (uint32_t)((len + kRound - 1) / kRound);
 		for (uint32_t r = 0; r < nr; r += 4) rgroups.push_back(make_int2(i, (int)r));
 		nrounds += nr;
-		blk_off[i] = nblk;
-		const uint32_t maxb = (uint32_t)(len / kBlockSyms) + 2;
-		for (uint32_t b = 0; b < maxb; b++) blk_desc.push_back(i);
-		nblk += maxb;
-		if (lp.func == 0) {
-			uint64_t dst = 0;
-			const bool cont = p->hist_kind == B200Z_HIST_CONTINUE;
-			const uint32_t *cum = (i < (int)p->sched_cum.size() && !p->sched_cum[i].empty()) ? p->sched_cum[i].data() : nullptr;
-			const int nch = cum ? (int)p->sched_cum[i].size() : 0;
-			const bool busy_last = !(i < (int)p->undrained.size() && p->undrained[i]);
-			StoredCarry cin{0, 0, 0, 0}, cout{0, 0, 0, 0};
-			if (cont) { // checked when the plan was created: stored_state is there
-				cin.strstart = p->stored_state[i].strstart;
-				cin.blockStart = p->stored_state[i].block_start;
-				cin.slides = p->stored_state[i].slides;
-				cin.inputOff = p->stored_state[i].input_off;
-			}
-			// (the carried state fixes where the data starts: pos_base is not needed, and may have any size)
-			const uint32_t start_bias = cont ? stored_rebase(cin, (uint32_t)H) : 0u;
-			int cut_call = 0;
-			stored_run((uint32_t)(len - H), cont ? 0u : (uint32_t)H, p->end_mode, [&](uint32_t start, uint32_t blen, bool last) {
-				sblocks.push_back(StoredBlock{i, start, blen, last ? 1u : 0u, dst});
-				dst += 5 + (uint64_t)blen;
-			}, cum, nch, cont ? &cin : nullptr, &cout, start_bias, busy_last, &cut_call);
-			if (p->end_mode == B200Z_END_NONE) // the data in front of the last block's end; none written: the entry state
-				p->stored_cut.push_back(make_uint2(sblocks.empty() || sblocks.back().stream != i ? 0u
-				                                                       : sblocks.back().src + sblocks.back().len - (uint32_t)H,
-				                                   (uint32_t)cut_call));
-			// what the window took in: everything, except when Finish() right behind an undrained SetInput makes
-			// DeflateStored end the stream early (lastBlock = finish although input is left, DeflaterEngine.cs:629-641);
-			// TotalIn and the Adler-32 of the reference then cover the consumed bytes only, and so do ours.  (Behind the
-			// cut of an open run the data starts strstart - blockStart bytes in front of inputOff.)
-			stored_taken[i] = (int64_t)(uint32_t)(cout.inputOff - (cont ? cin.inputOff - (uint32_t)(cin.strstart - cin.blockStart) : 0u));
-			if (p->stored_state) { // (behind an open run: the state at its cut)
-				p->stored_state[i].strstart = cout.strstart;
-				p->stored_state[i].block_start = cout.blockStart;
-				p->stored_state[i].slides = cout.slides;
-				p->stored_state[i].input_off = cout.inputOff;
-			}
-			slens.push_back((int64_t)dst);
+		z.entry[i] = RoundRec{(uint32_t)H, (uint32_t)kMinMatch - 1, 0u, 0u, (uint32_t)H, 0u};
+		if (!p->hist.empty()) {
+			hm_off[i] = (int64_t)hmask.size();
+			hmask.resize(hmask.size() + (size_t)H + 1, 0);
+			uint8_t *m = hmask.data() + hm_off[i];
+			if (!z.hist_mask[i].empty()) memcpy(m, z.hist_mask[i].data(), (size_t)H);
+			else if (H) m[H - 1] = 1, m[H > 1 ? H - 2 : 0] = 1; // the last two positions of a dictionary/segment are never inserted
 		}
 	}
 	rnd_off[n] = nrounds;
-	if (lp.func != 2) {
-		runs.clear();
-		tiles.clear();
-		chunks.clear();
-		rgroups.clear();
+	z.n_runs = (int)runs.size();
+	z.n_tiles = (int)tiles.size();
+	z.n_chunks = (int)chunks.size();
+	z.n_rgroups = (int)rgroups.size();
+	Arena &ws = p->ws;
+	const int64_t io = p->in_bytes;
+	z.o_run_desc = ws.upload(runs, 1);
+	z.o_tile_desc = ws.upload(tiles, 1);
+	z.o_hm_off = ws.upload(hm_off, 1);
+	z.o_hmask = ws.upload(hmask, 16);
+	z.o_link = ws.reserve<uint16_t>(io + 32);
+	z.o_mt = ws.reserve<uint2>(io + 8);
+	z.o_sym_local = ws.reserve<uint32_t>(io + 16);
+	z.o_chunks = ws.upload(chunks, 1);
+	z.o_rgroups = ws.upload(rgroups, 1);
+	z.o_rnd_off = ws.upload(rnd_off);
+	z.o_recs = ws.reserve<RoundRec>(nrounds + 1);
+	z.o_ents = ws.reserve<RoundRec>(nrounds + 1);
+	z.o_rnd_symoff = ws.reserve<uint32_t>(nrounds + 1);
+	z.o_entry = ws.upload(z.entry, 1);
+	z.o_cut = ws.reserve<RoundRec>(n + 1);
+	blocks_layout(p);
+	// lazy_launch: k_links, k_match, k_parse_chunk, k_parse_fix, k_parse_scan, k_parse_gather (+ k_parse_cut for an open
+	// run), then k_plan, k_scan, k_emit
+	p->launches = 9 + (p->end_mode == B200Z_END_NONE ? 1 : 0);
+}
+
+// stages: B200Z_STAGE_SEARCH = match finding (k_links, k_match), B200Z_STAGE_ENCODE = the parse
+static int lazy_launch(DeflatePlan *p, const uint8_t *d_in, cudaStream_t s, bool do_search, bool do_encode) {
+	const auto &z = p->lazy;
+	const Arena &ws = p->ws;
+	const int n = p->n;
+	const LevelParams lp = level_params(p->level);
+	const int64_t *in_off = ws.at(p->o_in_off), *in_len = ws.at(p->o_in_len);
+	uint16_t *link = ws.at(z.o_link);
+	uint2 *mt = ws.at(z.o_mt);
+	uint32_t *sym = ws.at(p->o_sym);
+	const uint32_t *hist = ws.at(p->o_hist);
+	const int64_t *bias = ws.at(p->o_bias);
+	if (do_search) {
+		p->mark(s, "k_links");
+		if (z.n_runs)
+			k_links<<<z.n_runs, kLinkThreads, kLinksSmem, s>>>(d_in, link, in_off, in_len, ws.at(z.o_run_desc), hist,
+			                                                   ws.at(z.o_hmask), ws.at(z.o_hm_off), (uint32_t)z.link_run);
+		p->mark(s, "k_match");
+		if (z.n_tiles)
+			k_match<<<z.n_tiles, kMatchThreads, kTileData + 2 * 2 * kTile, s>>>(d_in, link, mt, in_off, in_len,
+			                                                                   ws.at(z.o_tile_desc), hist, bias, sym, lp);
 	}
-	p->n_chunks = (int)chunks.size();
-	p->n_rgroups = (int)rgroups.size();
-	blk_off[n] = nblk;
+	if (!do_encode) return B200Z_OK;
+	p->mark(s, "k_parse");
+	uint32_t *sym_local = ws.at(z.o_sym_local);
+	const uint32_t *rnd_off = ws.at(z.o_rnd_off);
+	RoundRec *recs = ws.at(z.o_recs), *ents = ws.at(z.o_ents);
+	uint32_t *rnd_symoff = ws.at(z.o_rnd_symoff);
+	uint32_t *nsyms = ws.at(p->o_nsyms), *nblocks = ws.at(p->o_nblocks), *blk_off = ws.at(p->o_blk_off);
+	uint32_t *blk_start = ws.at(p->o_blk_start), *blk_ptop = ws.at(p->o_blk_ptop);
+	if (z.n_chunks)
+		k_parse_chunk<<<z.n_chunks, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, ws.at(z.o_chunks), rnd_off,
+		                                                 recs, ents, hist, bias, ws.at(z.o_entry), lp, p->strategy, parse_warm(),
+		                                                 p->end_mode);
+	k_parse_fix<<<n, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, rnd_off, recs, ents, z.parse_chunk, hist,
+	                                      bias, lp, p->strategy, p->end_mode);
+	k_parse_scan<<<n, 256, 0, s>>>(d_in, in_off, in_len, rnd_off, recs, rnd_symoff, sym, nsyms, nblocks, blk_off, blk_start,
+	                               blk_ptop, hist, p->end_mode);
+	if (z.n_rgroups)
+		k_parse_gather<<<z.n_rgroups, 128, 0, s>>>(sym_local, sym, in_off, in_len, ws.at(z.o_rgroups), rnd_off, recs,
+		                                           rnd_symoff, blk_off, blk_start, blk_ptop, hist);
+	if (p->end_mode == B200Z_END_NONE)
+		k_parse_cut<<<(n + 127) / 128, 128, 0, s>>>(d_in, link, mt, in_off, in_len, rnd_off, recs, rnd_symoff, nblocks, bias,
+		                                            ws.at(z.o_entry), ws.at(z.o_cut), n, lp, p->strategy);
+	return B200Z_OK;
+}
+
+// levels 1-4
+static void fast_layout(DeflatePlan *p, int64_t maxlen, int sms) {
+	auto &f = p->fast;
+	const int n = p->n;
+	// size of k_fast's prev[] table (see there)
+	const int64_t need = maxlen + 2;
+	f.prev_entries = 32768;
+	if (need <= 32768 && f.engine_state.empty()) f.prev_entries = (int)((need + 255) / 256 * 256); // (a carried state holds whole tables)
+	// persistent one-warp CTAs: as many per SM as their prev[] tables fit (head[] is in the pool), 16 at most
+	int per_sm = (int)((227 * 1024) / (2 * f.prev_entries + 1024));
+	if (per_sm > 16) per_sm = 16;
+	if (per_sm < 1) per_sm = 1;
+	const int64_t slots = (int64_t)sms * per_sm;
+	f.ctas = (int)(n < slots ? n : slots);
+	f.head_smem = n <= sms; // nothing to gain from sharing SMs: keep head[] next to prev[] (k_fast)
+	if (const char *e = getenv("B200Z_FAST_HEAD")) f.head_smem = e[0] == 's'; // "smem" / "pool": for tests and timing
+	Arena &ws = p->ws;
+	f.o_sched = ws.upload(p->sched, 1);
+	f.o_sched_off = ws.upload(p->sched_off);
+	f.o_undrained = ws.upload(p->undrained, 1);
+	f.o_state = ws.upload(f.engine_state.empty() ? std::vector<uint8_t *>(n) : f.engine_state, 1);
+	f.o_head = ws.reserve<uint16_t>(f.head_smem ? 128 : 32768ll * f.ctas);
+	f.o_counter = ws.reserve<uint32_t>(64);
+	f.o_cut = ws.reserve<uint2>(n + 1);
+	blocks_layout(p);
+	p->launches = 4; // k_fast, then k_plan, k_scan, k_emit (the memset of the CTA counter is not counted)
+}
+
+static int fast_launch(DeflatePlan *p, const uint8_t *d_in, cudaStream_t s) {
+	const auto &f = p->fast;
+	const Arena &ws = p->ws;
+	p->mark(s, "k_fast");
+	B200Z_CUDA(cudaMemsetAsync(ws.at(f.o_counter), 0, 4, s));
+	k_fast<<<f.ctas, 32, 2 * f.prev_entries + (f.head_smem ? 65536 : 0), s>>>(
+	    d_in, ws.at(p->o_sym), ws.at(p->o_in_off), ws.at(p->o_in_len), ws.at(p->o_nsyms), ws.at(p->o_nblocks), ws.at(p->o_blk_off),
+	    ws.at(p->o_blk_start), ws.at(p->o_blk_ptop), ws.at(p->o_hist), level_params(p->level), p->strategy, p->end_mode,
+	    f.prev_entries, ws.at(f.o_sched), ws.at(f.o_sched_off), ws.at(f.o_undrained), ws.at(f.o_state),
+	    p->hist_kind == B200Z_HIST_CONTINUE ? 1 : 0, fast_group_enabled(), p->n, f.head_smem ? nullptr : ws.at(f.o_head),
+	    ws.at(f.o_counter), ws.at(f.o_cut));
+	return B200Z_OK;
+}
+
+// level 0: the blocks DeflateStored writes follow from the lengths and the schedule alone.  Lowers ck_len to the bytes each
+// stream's window took in, and writes the state behind the run back to stored.state.
+static void stored_layout(DeflatePlan *p, std::vector<int64_t> &ck_len) {
+	auto &st = p->stored;
+	const int n = p->n;
+	const bool cont = p->hist_kind == B200Z_HIST_CONTINUE;
+	std::vector<StoredBlock> blocks;
+	std::vector<int64_t> lens;
+	for (int i = 0; i < n; i++) {
+		const int64_t len = p->in_len[i], H = hist_len(p, i);
+		uint64_t dst = 0;
+		const int nch = (int)(p->sched_off[i + 1] - p->sched_off[i]);
+		const uint32_t *cum = nch ? p->sched.data() + p->sched_off[i] : nullptr;
+		const bool busy_last = !p->undrained[i];
+		StoredCarry cin{0, 0, 0, 0}, cout{0, 0, 0, 0};
+		if (cont) // checked when the plan was created: stored.state is there
+			cin = StoredCarry{st.state[i].strstart, st.state[i].block_start, st.state[i].slides, st.state[i].input_off};
+		// (the carried state fixes where the data starts: pos_base is not needed, and may have any size)
+		const uint32_t start_bias = cont ? stored_rebase(cin, (uint32_t)H) : 0u;
+		int cut_call = 0;
+		stored_run((uint32_t)(len - H), cont ? 0u : (uint32_t)H, p->end_mode, [&](uint32_t start, uint32_t blen, bool last) {
+			blocks.push_back(StoredBlock{i, start, blen, last ? 1u : 0u, dst});
+			dst += 5 + (uint64_t)blen;
+		}, cum, nch, cont ? &cin : nullptr, &cout, start_bias, busy_last, &cut_call);
+		if (p->end_mode == B200Z_END_NONE) // the data in front of the last block's end; none written: the entry state
+			st.cut.push_back(make_uint2(blocks.empty() || blocks.back().stream != i ? 0u
+			                                                   : blocks.back().src + blocks.back().len - (uint32_t)H,
+			                            (uint32_t)cut_call));
+		// what the window took in: everything, except when Finish() right behind an undrained SetInput makes
+		// DeflateStored end the stream early (lastBlock = finish although input is left, DeflaterEngine.cs:629-641);
+		// TotalIn and the Adler-32 of the reference then cover the consumed bytes only, and so do ours.  (Behind the
+		// cut of an open run the data starts strstart - blockStart bytes in front of inputOff.)
+		const int64_t taken = (int64_t)(uint32_t)(cout.inputOff - (cont ? cin.inputOff - (uint32_t)(cin.strstart - cin.blockStart) : 0u));
+		if (taken < ck_len[i]) ck_len[i] = taken;
+		if (st.state) st.state[i] = b200z_stored_state{cout.strstart, cout.blockStart, cout.slides, cout.inputOff}; // (behind an open run: the state at its cut)
+		lens.push_back((int64_t)dst);
+	}
+	st.n_blocks = (int)blocks.size();
+	st.o_blocks = p->ws.upload(blocks, 1);
+	st.o_lens = p->ws.upload(lens, 1);
+	p->launches = 2; // k_stored, k_set_results
+}
+
+static void stored_launch(DeflatePlan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
+                          int64_t *d_out_bits, cudaStream_t s) {
+	const auto &st = p->stored;
+	const Arena &ws = p->ws;
+	p->mark(s, "k_stored");
+	if (st.n_blocks) k_stored<<<st.n_blocks, 256, 0, s>>>(d_in, d_out, ws.at(p->o_in_off), ws.at(p->o_out_off), ws.at(st.o_blocks));
+	k_set_results<<<(p->n + 127) / 128, 128, 0, s>>>(p->n, ws.at(st.o_lens), d_out_len, d_status, d_out_bits);
+}
+
+static int deflate_plan_build(DeflatePlan *p) {
+	const int n = p->n;
+	p->in_off.resize(n);
+	p->out_off.resize(n);
+	p->out_cap.resize(n);
+	std::vector<uint32_t> hist32(n);
+	std::vector<int64_t> ck_off(n), ck_len(n);
+	int64_t io = 0, oo = 0, maxlen = 0;
+	for (int i = 0; i < n; i++) {
+		const int64_t len = p->in_len[i], H = hist_len(p, i);
+		if (len < 0 || len > 0xFFFF0000ll) {
+			set_error("stream %d: length %lld out of range", i, (long long)len);
+			return B200Z_E_ARG;
+		}
+		hist32[i] = (uint32_t)H;
+		p->in_off[i] = io;
+		io += align_up(len + 16, kAlign);
+		p->out_off[i] = oo;
+		p->out_cap[i] = align_up(b200z_deflate_bound(len), kAlign);
+		oo += p->out_cap[i];
+		ck_off[i] = p->in_off[i] + H; // the checksum covers the data, never the history
+		ck_len[i] = len - H;
+		maxlen = len > maxlen ? len : maxlen;
+	}
 	p->in_bytes = io;
 	p->out_bytes = oo;
-	p->n_runs = (int)runs.size();
-	p->n_tiles = (int)tiles.size();
-	p->n_blkmax = (int)nblk;
 	Arena &ws = p->ws;
 	p->upload_streams(p->in_off, p->in_len, 0);
-	p->o_run_desc = ws.upload(runs, 1);
-	p->o_tile_desc = ws.upload(tiles, 1);
-	p->o_blk_desc = ws.upload(blk_desc, 1);
-	p->o_blk_off = ws.upload(blk_off);
-	p->o_nsyms = ws.reserve<uint32_t>(n);
-	p->o_nblocks = ws.reserve<uint32_t>(n);
-	p->o_blk_start = ws.reserve<uint32_t>(nblk + 1);
-	p->o_blk_ptop = ws.reserve<uint32_t>(nblk + 1);
-	p->o_meta = ws.reserve<BlockMeta>(nblk + 1);
-	p->o_tables = ws.reserve<BlockTables>(nblk + 1);
-	if (lp.func == 2) {
-		p->o_link = ws.reserve<uint16_t>(io + 32);
-		p->o_mt = ws.reserve<uint2>(io + 8);
-		p->o_sym_local = ws.reserve<uint32_t>(io + 16);
-		p->o_chunks = ws.upload(chunks, 1);
-		p->o_rgroups = ws.upload(rgroups, 1);
-		p->o_rnd_off = ws.upload(rnd_off);
-		p->o_recs = ws.reserve<RoundRec>(nrounds + 1);
-		p->o_ents = ws.reserve<RoundRec>(nrounds + 1);
-		p->o_rnd_symoff = ws.reserve<uint32_t>(nrounds + 1);
-		p->entry.resize(n);
-		for (int i = 0; i < n; i++) p->entry[i] = RoundRec{hist32[i], (uint32_t)kMinMatch - 1, 0u, 0u, hist32[i], 0u};
-		p->o_entry = ws.upload(p->entry, 1);
-		p->o_cut = ws.reserve<RoundRec>(n + 1);
-	}
-	if (lp.func != 0) p->o_sym = ws.reserve<uint32_t>(io + 16);
-	if (lp.func == 0) {
-		p->n_stored = (int)sblocks.size();
-		p->o_stored = ws.upload(sblocks, 1);
-		p->o_slens = ws.upload(slens, 1);
-	}
-	if (lp.func == 1) {
-		std::vector<uint32_t> sched_flat, sched_off(n + 1, 0u);
-		std::vector<int32_t> undrained32(n, 0);
-		std::vector<uint8_t *> fstate(n, nullptr);
-		for (int i = 0; i < n; i++) {
-			sched_off[i] = (uint32_t)sched_flat.size();
-			if (i < (int)p->sched_cum.size()) sched_flat.insert(sched_flat.end(), p->sched_cum[i].begin(), p->sched_cum[i].end());
-			if (i < (int)p->undrained.size()) undrained32[i] = p->undrained[i] ? 1 : 0;
-			if (i < (int)p->engine_state.size()) fstate[i] = static_cast<uint8_t *>(p->engine_state[i]);
-		}
-		sched_off[n] = (uint32_t)sched_flat.size();
-		p->o_sched = ws.upload(sched_flat, 1);
-		p->o_sched_off = ws.upload(sched_off);
-		p->o_undrained = ws.upload(undrained32, 1);
-		p->o_fstate = ws.upload(fstate, 1);
-		p->o_fhead = ws.reserve<uint16_t>(p->fast_head_smem ? 128 : 32768ll * p->fast_ctas);
-		p->o_fcounter = ws.reserve<uint32_t>(64);
-		p->o_fcut = ws.reserve<uint2>(n + 1);
-	}
 	p->o_hist = ws.upload(hist32, 1);
-	p->o_bias = ws.upload(bias64, 1);
-	p->o_bitbase = ws.upload(bitbase32, 1);
-	p->o_hm_off = ws.upload(hm_off, 1);
-	p->o_hmask = ws.upload(hmask, 16);
+	p->o_bias = ws.upload(p->bias, 1);
+	p->o_bitbase = ws.upload(p->bit_base, 1);
+	int sms = 0;
+	if (sm_count(&sms) != cudaSuccess) sms = 132;
+	switch (level_params(p->level).func) {
+	case 0: stored_layout(p, ck_len); break;
+	case 1: fast_layout(p, maxlen, sms); break;
+	default: lazy_layout(p, maxlen, sms);
+	}
 	if (p->wrap != B200Z_WRAP_RAW) {
-		std::vector<int64_t> ck_off(n), ck_len(n);
-		for (int i = 0; i < n; i++) { // the checksum covers the data, never the history
-			ck_off[i] = p->in_off[i] + hist32[i];
-			ck_len[i] = p->in_len[i] - hist32[i];
-			if (stored_taken[i] >= 0 && stored_taken[i] < ck_len[i]) ck_len[i] = stored_taken[i]; // level 0, see above
-		}
 		p->o_ck_off = ws.upload(ck_off, 1);
 		p->o_ck_len = ws.upload(ck_len, 1);
 		std::vector<CkTile> ck_tiles;
@@ -1876,14 +1965,13 @@ static int deflate_plan_build(DeflatePlan *p) {
 		p->n_ck_tiles = (int)ck_tiles.size();
 		p->o_ck_desc = ws.upload(ck_tiles, 1);
 		p->o_ck_acc = ws.reserve<unsigned long long>(2ll * (n + 1));
+		if (p->end_mode != B200Z_END_NONE) p->launches += 3; // checksum_launch (deflate_plan_run)
 	}
 	int rc = ws.alloc();
 	if (rc) return rc;
 	B200Z_CUDA(cudaFuncSetAttribute(k_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_links, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinksSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileData + 2 * 2 * kTile));
-	p->launches = (lp.func == 2 ? 9 : (lp.func == 1 ? 4 : 2)) + (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // + one memset node
-	if (p->end_mode == B200Z_END_NONE) p->launches += (lp.func == 2 ? 1 : 0) - (p->wrap != B200Z_WRAP_RAW ? 3 : 0); // k_parse_cut, no checksum
 	return B200Z_OK;
 }
 
@@ -1898,96 +1986,88 @@ int deflate_plan_create(int32_t n, const int64_t *in_len, int level, int strateg
 	p->wrap = wrap;
 	p->end_mode = end_mode;
 	p->in_len.assign(in_len, in_len + n);
-	if (end_mode == B200Z_END_NONE && level <= 4) {
-		// DeflateStored / DeflateFast carry window-relative tables across Deflate() calls that depend on the parse: the cut
-		// of a run goes to the engine state the plan writes (b200z_history.engine_state / stored_state)
-		bool have = hist && n > 0 && (level == 0 ? hist->stored_state != nullptr : hist->engine_state != nullptr);
+	static const b200z_history no_history{}; // (all NULL: what a plan without history reads)
+	if (!hist || n == 0) hist = &no_history;
+	const int kind = hist->kind;
+	if (level <= 4 && (end_mode == B200Z_END_NONE || kind == B200Z_HIST_CONTINUE)) {
+		// DeflateStored / DeflateFast keep window-relative tables across Deflate() calls that depend on the parse, not on the
+		// stream position: a stream that goes on after Flush() reads them from the run of the previous segment, and the cut
+		// of an open run writes them for the next one
+		bool have = (level == 0 ? hist->stored_state != nullptr : hist->engine_state != nullptr);
 		for (int i = 0; have && level >= 1 && i < n; i++) have = hist->engine_state[i] != nullptr;
 		if (!have) {
-			set_error("open runs (B200Z_END_NONE) at levels 0-4 need the engine state to write their cut into "
+			set_error("continuing a stream after Flush() and open runs (B200Z_END_NONE) at levels 0-4 need the engine state "
 			          "(b200z_history.engine_state / stored_state)");
 			return B200Z_E_UNSUPPORTED;
 		}
 	}
-	if (hist && n > 0 && level <= 4) {
-		// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
-		if (hist->chunk_count) {
-			if (!hist->chunk_len) {
-				set_error("history: chunk_count without chunk_len");
-				return B200Z_E_ARG;
-			}
-			p->sched_cum.resize(n);
-			for (int i = 0; i < n; i++) {
-				int64_t sum = 0;
-				for (int k = 0; k < hist->chunk_count[i]; k++) {
-					const int64_t c = hist->chunk_len[i] ? hist->chunk_len[i][k] : -1;
-					if (c < 0) {
-						set_error("stream %d: SetInput size %d", i, k);
-						return B200Z_E_ARG;
-					}
-					sum += c;
-					p->sched_cum[i].push_back((uint32_t)sum);
-				}
-				if (hist->chunk_count[i] < 0 || (hist->chunk_count[i] > 0 && sum != in_len[i])) {
-					set_error("stream %d: the SetInput sizes add up to %lld, the stream has %lld bytes", i, (long long)sum,
-					          (long long)in_len[i]);
+	// levels 0-4: the call pattern and the engine state between segments (header: "streams with history")
+	const bool sched = level <= 4 && hist->chunk_count;
+	if (sched && !hist->chunk_len) {
+		set_error("history: chunk_count without chunk_len");
+		return B200Z_E_ARG;
+	}
+	if (kind != B200Z_HIST_NONE && ((kind != B200Z_HIST_DICTIONARY && kind != B200Z_HIST_CONTINUE) || !hist->hist_len)) {
+		set_error("history: kind/hist_len");
+		return B200Z_E_ARG;
+	}
+	p->hist_kind = kind;
+	p->check_seeded = kind != B200Z_HIST_NONE && hist->check_seeded != 0;
+	if (kind != B200Z_HIST_NONE) p->hist.assign(hist->hist_len, hist->hist_len + n);
+	p->bias.assign(n, 0);
+	p->bit_base.assign(n, 0u);
+	p->lazy.hist_mask.resize(n);
+	p->sched_off.assign(n + 1, 0u);
+	p->undrained.assign(n, 0);
+	if (hist->engine_state) p->fast.engine_state.resize(n);
+	p->stored.state = hist->stored_state;
+	for (int i = 0; i < n; i++) {
+		if (sched) {
+			int64_t sum = 0;
+			for (int k = 0; k < hist->chunk_count[i]; k++) {
+				const int64_t c = hist->chunk_len[i] ? hist->chunk_len[i][k] : -1;
+				if (c < 0) {
+					set_error("stream %d: SetInput size %d", i, k);
 					return B200Z_E_ARG;
 				}
+				sum += c;
+				p->sched.push_back((uint32_t)sum);
+			}
+			if (hist->chunk_count[i] < 0 || (hist->chunk_count[i] > 0 && sum != in_len[i])) {
+				set_error("stream %d: the SetInput sizes add up to %lld, the stream has %lld bytes", i, (long long)sum,
+				          (long long)in_len[i]);
+				return B200Z_E_ARG;
 			}
 		}
-		if (hist->undrained_last) p->undrained.assign(hist->undrained_last, hist->undrained_last + n);
-		if (hist->engine_state && level >= 1) p->engine_state.assign(hist->engine_state, hist->engine_state + n);
-		if (hist->stored_state && level == 0) p->stored_state = hist->stored_state;
-	}
-	if (hist && hist->kind != B200Z_HIST_NONE && n > 0) {
-		if ((hist->kind != B200Z_HIST_DICTIONARY && hist->kind != B200Z_HIST_CONTINUE) || !hist->hist_len) {
-			set_error("history: kind/hist_len");
+		p->sched_off[i + 1] = (uint32_t)p->sched.size();
+		p->undrained[i] = hist->undrained_last && hist->undrained_last[i] ? 1 : 0;
+		if (hist->engine_state) p->fast.engine_state[i] = static_cast<uint8_t *>(hist->engine_state[i]);
+		if (kind == B200Z_HIST_NONE) continue;
+		const int64_t H = p->hist[i];
+		if (H < 0 || H > 32768 || (kind == B200Z_HIST_DICTIONARY && H > kMaxDist)) {
+			set_error("stream %d: history of %lld bytes (at most %d)", i, (long long)H, kind == B200Z_HIST_DICTIONARY ? kMaxDist : 32768);
 			return B200Z_E_ARG;
 		}
-		if (hist->kind == B200Z_HIST_CONTINUE && level < 5) {
-			// DeflateStored / DeflateFast keep window-relative state across Deflate() calls that is not a function of the
-			// stream position: it has to come from the run of the previous segment
-			bool have = level == 0 ? p->stored_state != nullptr : !p->engine_state.empty();
-			for (void *q : p->engine_state) have = have && q != nullptr;
-			if (!have) {
-				set_error("continuing a stream after Flush() at levels 0-4 needs the engine state of the previous segment "
-				          "(b200z_history.engine_state / stored_state)");
-				return B200Z_E_UNSUPPORTED;
-			}
+		int64_t pos_base = (hist->pos_base && kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
+		const int32_t bit_base = hist->bit_base ? hist->bit_base[i] : 0;
+		// (levels 0-4 keep positions relative to the carried engine state: carry_rebase)
+		if (pos_base < H || bit_base < 0 || bit_base > 7) {
+			set_error("stream %d: pos_base/bit_base", i);
+			return B200Z_E_ARG;
 		}
-		p->hist_kind = hist->kind;
-		p->check_seeded = hist->check_seeded != 0;
-		p->hist.assign(hist->hist_len, hist->hist_len + n);
-		p->pos_base.resize(n);
-		p->bit_base.resize(n);
-		p->hist_mask.resize(n);
-		for (int i = 0; i < n; i++) {
-			const int64_t H = p->hist[i];
-			if (H < 0 || H > 32768 || (hist->kind == B200Z_HIST_DICTIONARY && H > kMaxDist)) {
-				set_error("stream %d: history of %lld bytes (at most %d)", i, (long long)H,
-				          hist->kind == B200Z_HIST_DICTIONARY ? kMaxDist : 32768);
-				return B200Z_E_ARG;
-			}
-			p->pos_base[i] = (hist->pos_base && hist->kind == B200Z_HIST_CONTINUE) ? hist->pos_base[i] : H;
-			p->bit_base[i] = hist->bit_base ? hist->bit_base[i] : 0;
-			// (levels 0-4 keep positions relative to the carried engine state: carry_rebase)
-			if (p->pos_base[i] < H || p->bit_base[i] < 0 || p->bit_base[i] > 7) {
-				set_error("stream %d: pos_base/bit_base", i);
-				return B200Z_E_ARG;
-			}
-			// Levels 5-9 read the position only through the window phase, which is periodic with 32768 from kSlideFirst on
-			// (is_slide_pos, slides_done; storedOffset moves with both): the equal phase in the first period keeps the
-			// kernels' 32-bit positions valid in a stream of any length
-			if (level >= 5 && p->pos_base[i] >= (int64_t)kSlideFirst)
-				p->pos_base[i] = (int64_t)kSlideFirst + (p->pos_base[i] - (int64_t)kSlideFirst) % 32768;
-			if (level >= 5 && p->pos_base[i] + in_len[i] > 0xFFFFFFFFll) {
-				set_error("stream %d: %lld bytes behind position %lld do not fit one plan slot", i, (long long)in_len[i],
-				          (long long)p->pos_base[i]);
-				return B200Z_E_ARG;
-			}
-			if (hist->hist_mask && hist->hist_mask[i]) p->hist_mask[i].assign(hist->hist_mask[i], hist->hist_mask[i] + H);
-			p->in_len[i] += H; // the input slot holds history + data
+		// Levels 5-9 read the position only through the window phase, which is periodic with 32768 from kSlideFirst on
+		// (is_slide_pos, slides_done; storedOffset moves with both): the equal phase in the first period keeps the
+		// kernels' 32-bit positions valid in a stream of any length
+		if (level >= 5 && pos_base >= (int64_t)kSlideFirst) pos_base = (int64_t)kSlideFirst + (pos_base - (int64_t)kSlideFirst) % 32768;
+		if (level >= 5 && pos_base + in_len[i] > 0xFFFFFFFFll) {
+			set_error("stream %d: %lld bytes behind position %lld do not fit one plan slot", i, (long long)in_len[i],
+			          (long long)pos_base);
+			return B200Z_E_ARG;
 		}
+		p->bias[i] = pos_base - H;
+		p->bit_base[i] = (uint32_t)bit_base;
+		if (hist->hist_mask && hist->hist_mask[i]) p->lazy.hist_mask[i].assign(hist->hist_mask[i], hist->hist_mask[i] + H);
+		p->in_len[i] += H; // the input slot holds history + data
 	}
 	const int rc = deflate_plan_build(p.get());
 	if (rc == B200Z_OK) *out = p.release();
@@ -2000,21 +2080,7 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 	const Arena &ws = p->ws;
 	const int n = p->n;
 	if (n == 0) return B200Z_OK;
-	const LevelParams lp = level_params(p->level);
-	const int64_t *in_off = ws.at(p->o_in_off), *in_len = ws.at(p->o_in_len);
-	const int64_t *out_off = ws.at(p->o_out_off), *out_cap = ws.at(p->o_out_cap);
-	uint16_t *link = lp.func == 2 ? ws.at(p->o_link) : nullptr;
-	uint2 *mt = lp.func == 2 ? ws.at(p->o_mt) : nullptr;
-	uint32_t *sym = lp.func != 0 ? ws.at(p->o_sym) : nullptr;
-	uint32_t *nsyms = ws.at(p->o_nsyms), *nblocks = ws.at(p->o_nblocks);
-	uint32_t *blk_off = ws.at(p->o_blk_off);
-	int32_t *blk_desc = ws.at(p->o_blk_desc);
-	uint32_t *blk_start = ws.at(p->o_blk_start), *blk_ptop = ws.at(p->o_blk_ptop);
-	BlockMeta *meta = ws.at(p->o_meta);
-	BlockTables *tables = ws.at(p->o_tables);
-	const uint32_t *hist = ws.at(p->o_hist), *bit_base = ws.at(p->o_bitbase);
-	const int64_t *bias = ws.at(p->o_bias);
-
+	const int func = level_params(p->level).func;
 	// stages: B200Z_STAGE_SEARCH = match finding (levels 5-9: k_links, k_match), B200Z_STAGE_ENCODE = everything else.
 	// Splitting lets a caller put other work (e.g. an inflate plan on a second stream) next to the ENCODE kernels, which
 	// leave most of an SM's shared memory free, instead of next to k_match, which takes all of it.
@@ -2026,77 +2092,42 @@ int deflate_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int6
 		bool v;
 		~TimingRestore() { p->timing = v; }
 	} timing_restore{p, was_timing};
-	if (lp.func != 2 && !do_encode) return B200Z_OK; // levels 0-4 have no separate search stage
+	if (func != 2 && !do_encode) return B200Z_OK; // levels 0-4 have no separate search stage
 	p->ev_used = 0;
-	if (lp.func == 0) {
-		// level 0: stored blocks laid out when the plan was built
-		p->mark(s, "k_stored");
-		if (p->n_stored) k_stored<<<p->n_stored, 256, 0, s>>>(d_in, d_out, in_off, out_off, ws.at(p->o_stored));
-		k_set_results<<<(n + 127) / 128, 128, 0, s>>>(n, ws.at(p->o_slens), d_out_len, d_status, d_out_bits);
-		if (p->end_mode == B200Z_END_NONE) p->cut_ready = true;
+	if (func == 0) {
+		stored_launch(p, d_in, d_out, d_out_len, d_status, d_out_bits, s);
 	} else {
 		if (do_encode) {
 			p->mark(s, "memset");
 			B200Z_CUDA(cudaMemsetAsync(d_out, 0, (size_t)p->out_bytes, s));
 		}
-		if (lp.func == 1) {
-			p->mark(s, "k_fast");
-			B200Z_CUDA(cudaMemsetAsync(ws.at(p->o_fcounter), 0, 4, s));
-			k_fast<<<p->fast_ctas, 32, 2 * p->fast_prev_entries + (p->fast_head_smem ? 65536 : 0), s>>>(
-			    d_in, sym, in_off, in_len, nsyms, nblocks, blk_off, blk_start, blk_ptop, hist, lp, p->strategy, p->end_mode,
-			    p->fast_prev_entries, ws.at(p->o_sched), ws.at(p->o_sched_off), ws.at(p->o_undrained), ws.at(p->o_fstate),
-			    p->hist_kind == B200Z_HIST_CONTINUE ? 1 : 0, fast_group_enabled(), n, p->fast_head_smem ? nullptr : ws.at(p->o_fhead),
-			    ws.at(p->o_fcounter), ws.at(p->o_fcut));
-			if (p->end_mode == B200Z_END_NONE) p->cut_ready = true;
-		} else {
-			if (do_search) {
-				p->mark(s, "k_links");
-				if (p->n_runs)
-					k_links<<<p->n_runs, kLinkThreads, kLinksSmem, s>>>(d_in, link, in_off, in_len, ws.at(p->o_run_desc), hist,
-					                                                    ws.at(p->o_hmask), ws.at(p->o_hm_off), (uint32_t)p->link_run);
-				p->mark(s, "k_match");
-				if (p->n_tiles)
-					k_match<<<p->n_tiles, kMatchThreads, kTileData + 2 * 2 * kTile, s>>>(d_in, link, mt, in_off, in_len,
-					                                                                   ws.at(p->o_tile_desc), hist, bias, sym, lp);
-			}
-			if (!do_encode) {
-				B200Z_CUDA(cudaGetLastError());
-				return B200Z_OK;
-			}
-			p->mark(s, "k_parse");
-			uint32_t *sym_local = ws.at(p->o_sym_local);
-			const uint32_t *rnd_off = ws.at(p->o_rnd_off);
-			RoundRec *recs = ws.at(p->o_recs), *ents = ws.at(p->o_ents);
-			uint32_t *rnd_symoff = ws.at(p->o_rnd_symoff);
-			if (p->n_chunks)
-				k_parse_chunk<<<p->n_chunks, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, ws.at(p->o_chunks), rnd_off,
-				                                                 recs, ents, hist, bias, ws.at(p->o_entry), lp, p->strategy, parse_warm(),
-				                                                 p->end_mode);
-			k_parse_fix<<<n, 32, kParseSmem, s>>>(d_in, link, mt, sym_local, in_off, in_len, rnd_off, recs, ents, p->parse_chunk, hist,
-			                                      bias, lp, p->strategy, p->end_mode);
-			k_parse_scan<<<n, 256, 0, s>>>(d_in, in_off, in_len, rnd_off, recs, rnd_symoff, sym, nsyms, nblocks, blk_off, blk_start,
-			                               blk_ptop, hist, p->end_mode);
-			if (p->n_rgroups)
-				k_parse_gather<<<p->n_rgroups, 128, 0, s>>>(sym_local, sym, in_off, in_len, ws.at(p->o_rgroups), rnd_off, recs,
-				                                           rnd_symoff, blk_off, blk_start, blk_ptop, hist);
-			if (p->end_mode == B200Z_END_NONE) {
-				k_parse_cut<<<(n + 127) / 128, 128, 0, s>>>(d_in, link, mt, in_off, in_len, rnd_off, recs, rnd_symoff, nblocks, bias,
-				                                            ws.at(p->o_entry), ws.at(p->o_cut), n, lp, p->strategy);
-				p->cut_ready = true;
-			}
+		const int rc = func == 1 ? fast_launch(p, d_in, s) : lazy_launch(p, d_in, s, do_search, do_encode);
+		if (rc) return rc;
+		if (!do_encode) {
+			B200Z_CUDA(cudaGetLastError());
+			return B200Z_OK;
 		}
+		// Huffman trees per block, block offsets, the bits
+		const int64_t *in_off = ws.at(p->o_in_off), *out_off = ws.at(p->o_out_off);
+		uint32_t *sym = ws.at(p->o_sym), *nblocks = ws.at(p->o_nblocks), *blk_off = ws.at(p->o_blk_off);
+		int32_t *blk_desc = ws.at(p->o_blk_desc);
+		BlockMeta *meta = ws.at(p->o_meta);
+		BlockTables *tables = ws.at(p->o_tables);
 		p->mark(s, "k_plan");
-		k_plan<<<p->n_blkmax, kPlanThreads, 0, s>>>(sym, in_off, in_len, nsyms, nblocks, blk_off, blk_desc, blk_start, blk_ptop,
-		                                            meta, tables, bias, p->end_mode);
+		k_plan<<<p->n_blkmax, kPlanThreads, 0, s>>>(sym, in_off, ws.at(p->o_in_len), ws.at(p->o_nsyms), nblocks, blk_off, blk_desc,
+		                                            ws.at(p->o_blk_start), ws.at(p->o_blk_ptop), meta, tables, ws.at(p->o_bias),
+		                                            p->end_mode);
 		p->mark(s, "k_scan");
-		k_scan<<<(n + 127) / 128, 128, 0, s>>>(n, nblocks, blk_off, meta, d_out, out_off, out_cap, d_out_len, d_status,
-		                                       d_out_bits, bit_base, p->end_mode);
+		k_scan<<<(n + 127) / 128, 128, 0, s>>>(n, nblocks, blk_off, meta, d_out, out_off, ws.at(p->o_out_cap), d_out_len, d_status,
+		                                       d_out_bits, ws.at(p->o_bitbase), p->end_mode);
 		p->mark(s, "k_emit");
 		k_emit<<<p->n_blkmax, 256, 0, s>>>(d_in, sym, d_out, in_off, out_off, nblocks, blk_off, blk_desc, meta, tables);
 	}
 	p->mark(s, "checksum");
 	// (an open run leaves the running checksum alone: its caller knows which of the bytes the run covered)
-	if (p->wrap != B200Z_WRAP_RAW && d_check && p->end_mode != B200Z_END_NONE) {
+	if (p->end_mode == B200Z_END_NONE) {
+		p->cut_ready = true;
+	} else if (p->wrap != B200Z_WRAP_RAW && d_check) {
 		int rc = checksum_launch(p->wrap == B200Z_WRAP_ZLIB ? 1 : 0, d_in, ws.at(p->o_ck_off), ws.at(p->o_ck_len), n,
 		                         ws.at(p->o_ck_desc), p->n_ck_tiles, ws.at(p->o_ck_acc), d_check, p->check_seeded ? 0 : 1, s, false);
 		if (rc) return rc;
@@ -2112,10 +2143,10 @@ int deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry) {
 		set_error("entry states are for levels 5-9");
 		return B200Z_E_UNSUPPORTED;
 	}
-	std::vector<RoundRec> v(p->entry);
+	std::vector<RoundRec> v(p->lazy.entry);
 	for (int i = 0; i < p->n; i++) {
 		const b200z_parse_entry &e = entry[i];
-		const int64_t H = p->hist.empty() ? 0 : p->hist[i];
+		const int64_t H = hist_len(p, i);
 		const int64_t data = p->in_len[i] - H;
 		const bool pending = e.match_len >= kMinMatch;
 		// with nothing pending matchLen is MIN_MATCH - 1; a byte left pending lies in the data, and so does its match
@@ -2131,19 +2162,19 @@ int deflate_plan_set_entry(b200z_plan *plan, const b200z_parse_entry *entry) {
 		v[i].mstart = pending ? (uint32_t)(H - e.match_dist) : 0u;
 		v[i].prevAvail = (uint32_t)e.prev_available;
 	}
-	const int rc = p->ws.write(p->o_entry, v);
-	if (rc == B200Z_OK) p->entry = v;
+	const int rc = p->ws.write(p->lazy.o_entry, v);
+	if (rc == B200Z_OK) p->lazy.entry = v;
 	return rc;
 }
 
 // levels 0-4: per stream (covered, SetInput call) of the last cut
 static int fast_cuts(DeflatePlan *p, std::vector<uint2> &v, cudaStream_t s) {
 	if (p->level == 0) {
-		v = p->stored_cut;
+		v = p->stored.cut;
 		return B200Z_OK;
 	}
 	v.resize((size_t)p->n);
-	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->o_fcut), sizeof(uint2) * v.size(), cudaMemcpyDeviceToHost, s));
+	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->fast.o_cut), sizeof(uint2) * v.size(), cudaMemcpyDeviceToHost, s));
 	B200Z_CUDA(cudaStreamSynchronize(s));
 	return B200Z_OK;
 }
@@ -2165,10 +2196,10 @@ int deflate_plan_get_cut(b200z_plan *plan, int64_t *covered, b200z_parse_entry *
 		return B200Z_OK;
 	}
 	std::vector<RoundRec> v((size_t)p->n);
-	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->o_cut), sizeof(RoundRec) * v.size(), cudaMemcpyDeviceToHost, s));
+	B200Z_CUDA(cudaMemcpyAsync(v.data(), p->ws.at(p->lazy.o_cut), sizeof(RoundRec) * v.size(), cudaMemcpyDeviceToHost, s));
 	B200Z_CUDA(cudaStreamSynchronize(s));
 	for (int i = 0; i < p->n; i++) {
-		const int64_t H = p->hist.empty() ? 0 : p->hist[i];
+		const int64_t H = hist_len(p, i);
 		const int64_t pos = (int64_t)v[i].p - v[i].prevAvail; // the first byte not written
 		covered[i] = pos - H;
 		next[i].prev_available = (int32_t)v[i].prevAvail;
