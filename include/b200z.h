@@ -244,9 +244,21 @@ int b200z_plan_run(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int64_
 int b200z_plan_run_stages(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                           uint32_t *d_check, int64_t *d_in_used, int stages, void *cuda_stream);
 
+/* ---- LZW (.Z, Unix compress): LzwInputStream (Lzw/LzwInputStream.cs) for n independent streams ----
+ * A plan of kind 2: stream i is comp_len[i] bytes (the 3-byte header included, at most 2^31 - 1) and decodes into at
+ * most out_cap[i] bytes.  It runs through b200z_plan_run: d_out_len[i] gets the bytes in front of the first bad code (all
+ * of them for a good stream), d_status[i] = code | detail << 8 (INTEGRATION.md §2), d_check[i] (may be NULL) the numbers the
+ * reference's message quotes, d_in_used[i] (may be NULL) the bytes up to the last code read.  .Z has no size field: a
+ * stream whose output does not fit out_cap gets B200Z_E_NOMEM, nothing is written and d_out_len[i] is the size it needs;
+ * NOMEM takes the place of a B200Z_E_DATA / B200Z_E_INTERNAL status the stream also has (the bytes in front of its bad code
+ * did not fit), and a run with a large enough out_cap reports that one.
+ * b200z_plan_get_stats gives the epochs (CLEARs + 1), the codes and the longest string of the last run. */
+int b200z_lzw_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, b200z_plan **plan);
+
 /* Packs the streams a run produced back to back (16-byte aligned starts) into d_packed, so a caller copies only the
  * produced bytes to the host: d_packed_off[n + 1] (device) receives the start of every stream and, last, the total.
- * d_packed needs b200z_plan_out_bytes() of room.  Asynchronous on `stream`. */
+ * d_packed needs b200z_plan_out_bytes() of room.  Asynchronous on `stream`.  LZW plans: B200Z_E_UNSUPPORTED (a stream that
+ * did not fit reports the size it needs in d_out_len). */
 int b200z_plan_pack(b200z_plan *plan, const uint8_t *d_out, const int64_t *d_out_len, uint8_t *d_packed,
                     int64_t *d_packed_off, void *cuda_stream);
 
@@ -301,6 +313,13 @@ int b200z_deflate_batch_multi(const int32_t *devices, int32_t n_devices, const u
 int b200z_inflate_batch_multi(const int32_t *devices, int32_t n_devices, const uint8_t *const *in, const int64_t *in_len, int32_t n,
                               int wrap, uint8_t *const *out, const int64_t *out_cap, int64_t *out_len, int64_t *in_used,
                               uint32_t *check, int32_t *status);
+/* LZW pipelines and batch calls (b200z_lzw_plan_create); value[i] (may be NULL) = the numbers of stream i's error message */
+int b200z_lzw_pipeline_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int depth, b200z_pipeline **pipe);
+int b200z_lzw_batch(const uint8_t *const *in, const int64_t *in_len, int32_t n, uint8_t *const *out, const int64_t *out_cap,
+                    int64_t *out_len, int64_t *in_used, uint32_t *value, int32_t *status);
+int b200z_lzw_batch_multi(const int32_t *devices, int32_t n_devices, const uint8_t *const *in, const int64_t *in_len, int32_t n,
+                          uint8_t *const *out, const int64_t *out_cap, int64_t *out_len, int64_t *in_used, uint32_t *value,
+                          int32_t *status);
 /* worst-case compressed size for `len` input bytes at any level (capacity a caller should provide) */
 int64_t b200z_deflate_bound(int64_t len);
 

@@ -330,6 +330,17 @@ int b200z_inflate_plan_create_ex(int32_t n, const int64_t *comp_len, const int64
 	return inflate_plan_create(n, comp_len, out_cap, wrap, dict_len, plan);
 }
 
+int b200z_lzw_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, b200z_plan **plan) {
+	if (!plan || n < 0 || (n > 0 && (!comp_len || !out_cap))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	int rc = ensure_init();
+	if (rc) return rc;
+	DeviceGuard guard(current_device());
+	return lzw_plan_create(n, comp_len, out_cap, plan);
+}
+
 int b200z_inflate_plan_set_start_bits(b200z_plan *plan, const int32_t *start_bit) {
 	DeviceGuard guard(plan ? plan->device : -1);
 	if (!plan || plan->kind != 1 || (plan->n > 0 && !start_bit)) {
@@ -400,10 +411,11 @@ int b200z_plan_get_resume_points(b200z_plan *plan, int64_t *hdr_bit, int64_t *bo
 
 int b200z_plan_get_stats(b200z_plan *plan, uint32_t *v, int32_t cap, void *cuda_stream) {
 	DeviceGuard guard(plan ? plan->device : -1);
-	if (!plan || plan->kind != 1 || !v || cap < 0) {
+	if (!plan || plan->kind == 0 || !v || cap < 0) {
 		set_error("bad arguments");
 		return B200Z_E_ARG;
 	}
+	if (plan->kind == 2) return lzw_plan_stats(plan, v, cap, (cudaStream_t)cuda_stream);
 	return inflate_plan_stats(plan, v, cap, (cudaStream_t)cuda_stream);
 }
 
@@ -466,7 +478,8 @@ int b200z_plan_run_stages(b200z_plan *plan, const uint8_t *d_in, uint8_t *d_out,
 	}
 	cudaStream_t s = (cudaStream_t)cuda_stream;
 	if (plan->kind == 0) return deflate_plan_run(plan, d_in, d_out, d_out_len, d_status, d_check, d_in_used, s, stages);
-	if (!(stages & B200Z_STAGE_ENCODE)) return B200Z_OK; // an inflate plan is a single stage
+	if (!(stages & B200Z_STAGE_ENCODE)) return B200Z_OK; // inflate and LZW plans are a single stage
+	if (plan->kind == 2) return lzw_plan_run(plan, d_in, d_out, d_out_len, d_status, d_check, d_in_used, s);
 	return inflate_plan_run(plan, d_in, d_out, d_out_len, d_status, d_check, d_in_used, s);
 }
 
@@ -476,6 +489,10 @@ int b200z_plan_pack(b200z_plan *plan, const uint8_t *d_out, const int64_t *d_out
 	if (!plan || !d_out || !d_out_len || !d_packed || !d_packed_off) {
 		set_error("bad arguments");
 		return B200Z_E_ARG;
+	}
+	if (plan->kind == 2) { // a stream that did not fit reports the size it needs in d_out_len, not bytes in d_out
+		set_error("LZW plans are not packed: a B200Z_E_NOMEM stream's out_len is the size it needs, not bytes of its slot");
+		return B200Z_E_UNSUPPORTED;
 	}
 	if (plan->n == 0) return B200Z_OK;
 	cudaStream_t s = (cudaStream_t)cuda_stream;

@@ -65,6 +65,19 @@ const char *inflate_detail_msg(int detail) {
 	}
 }
 
+std::string lzw_detail_msg(int32_t status, uint32_t value) {
+	char b[160];
+	switch ((status >> 8) & 0xFF) {
+	case 32: snprintf(b, sizeof b, "Wrong LZW header. Magic bytes don't match. 0x%02x 0x%02x", value >> 8, value & 0xFF); break;
+	case 33: snprintf(b, sizeof b, "Stream compressed with %u bits, but decompression can only handle 16 bits.", value); break;
+	case 34: snprintf(b, sizeof b, "Unsupported bits set in the header."); break;
+	case 35: snprintf(b, sizeof b, "corrupt input: %u > 255", value); break;
+	case 36: snprintf(b, sizeof b, "corrupt input: code=%u, freeEnt=%u", value >> 16, value & 0xFFFF); break;
+	default: snprintf(b, sizeof b, "LZW stream: the reference fails with a non-SharpZip exception (status detail %d)", (status >> 8) & 0xFF);
+	}
+	return b;
+}
+
 // One run of a handle's single-stream plan on the legacy default stream; returns with the run's metadata in st.h and the
 // produced bytes in st.hout at the stream's out_off.  `in` is the handle's own pageable copy of the input.
 static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const uint32_t *check_seed) {

@@ -108,9 +108,14 @@ int stage_run(b200z_plan *plan, Staging &st, const uint8_t *const *in, bool in_p
 	return B200Z_OK;
 }
 
+// the bytes a run wrote for stream i: an LZW stream that did not fit reports the size it needs and wrote nothing
+static int64_t produced(const b200z_plan *plan, const PipeMeta &m, int i) {
+	return plan->kind == 2 && (m.status[i] & 0xFF) == B200Z_E_NOMEM ? 0 : m.out_len[i];
+}
+
 int streams_down(const b200z_plan *plan, Staging &st, uint8_t *const *dst, cudaStream_t s) {
 	for (int i = 0; i < plan->n; i++) {
-		const int64_t L = st.h.out_len[i];
+		const int64_t L = produced(plan, st.h, i);
 		if (L > 0)
 			B200Z_CUDA(cudaMemcpyAsync(dst ? dst[i] : st.hout.p + plan->out_off[(size_t)i], st.dout.p + plan->out_off[(size_t)i], (size_t)L,
 			                           cudaMemcpyDeviceToHost, s));
@@ -222,12 +227,13 @@ static int multi_batch(int kind, const int32_t *devices, int32_t n_devices, cons
 		const int a = first[(size_t)d], cnt = first[(size_t)d + 1] - a;
 		if (cnt == 0) continue;
 		PipeKey key{devices[d], kind, cnt, level, strategy, wrap, end_mode, std::vector<int64_t>(in_len + a, in_len + a + cnt),
-		            kind == 1 ? std::vector<int64_t>(out_cap + a, out_cap + a + cnt) : std::vector<int64_t>()};
+		            kind != 0 ? std::vector<int64_t>(out_cap + a, out_cap + a + cnt) : std::vector<int64_t>()};
 		b200z_pipeline *p = g_pipes.find(key);
 		if (!p) {
 			if ((rc = b200z_init(devices[d]))) { result = rc; break; } // (makes the device this thread's current one for the creation)
-			rc = kind == 0 ? b200z_deflate_pipeline_create(cnt, in_len + a, level, strategy, wrap, end_mode, 1, &p)
-			               : b200z_inflate_pipeline_create(cnt, in_len + a, out_cap + a, wrap, 1, &p);
+			rc = kind == 0   ? b200z_deflate_pipeline_create(cnt, in_len + a, level, strategy, wrap, end_mode, 1, &p)
+			     : kind == 1 ? b200z_inflate_pipeline_create(cnt, in_len + a, out_cap + a, wrap, 1, &p)
+			                 : b200z_lzw_pipeline_create(cnt, in_len + a, out_cap + a, 1, &p);
 			if (rc) { result = rc; break; }
 			g_pipes.put(std::move(key), p);
 		}
@@ -280,6 +286,17 @@ int b200z_inflate_pipeline_create(int32_t n, const int64_t *comp_len, const int6
 	int rc = b200z_inflate_plan_create(n, comp_len, out_cap, wrap, &plan);
 	if (rc) return rc;
 	return pipeline_finish_create(plan, wrap, depth, pipe);
+}
+
+int b200z_lzw_pipeline_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, int depth, b200z_pipeline **pipe) {
+	if (!pipe) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	b200z_plan *plan = nullptr;
+	int rc = b200z_lzw_plan_create(n, comp_len, out_cap, &plan);
+	if (rc) return rc;
+	return pipeline_finish_create(plan, B200Z_WRAP_RAW, depth, pipe);
 }
 
 int b200z_pipeline_destroy(b200z_pipeline *p) {
@@ -396,24 +413,25 @@ int b200z_pipeline_collect(b200z_pipeline *p, uint8_t *const *out, const int64_t
 			}
 		});
 	} else {
-		// ---- inflate: every stream's produced bytes; straight into the caller's buffers when CUDA knows them as pinned ----
+		// ---- inflate and LZW: every stream's produced bytes; straight into the caller's buffers when CUDA knows them as
+		// pinned.  An LZW stream that needs more than its capacity reports B200Z_E_NOMEM and the size it needs in out_len. ----
 		bool all_pinned = n > 0;
 		for (int i = 0; i < n && all_pinned; i++)
-			if (sl.h.out_len[i] > 0 && (i < 4 || (i & 63) == 0)) all_pinned = host_ptr_is_pinned(out[i]);
+			if (produced(plan, sl.h, i) > 0 && (i < 4 || (i & 63) == 0)) all_pinned = host_ptr_is_pinned(out[i]);
 		int rc = streams_down(plan, sl, all_pinned ? out : nullptr, p->s_down);
 		if (rc) return rc;
-		for (int i = 0; i < n; i++) moved += sl.h.out_len[i];
+		for (int i = 0; i < n; i++) moved += produced(plan, sl.h, i);
 		if (!all_pinned)
 			host_parallel_for(n, moved, [&](int a, int b) {
 				for (int i = a; i < b; i++)
-					if (sl.h.out_len[i] > 0) memcpy(out[i], sl.hout.p + plan->out_off[(size_t)i], (size_t)sl.h.out_len[i]);
+					if (produced(plan, sl.h, i) > 0) memcpy(out[i], sl.hout.p + plan->out_off[(size_t)i], (size_t)produced(plan, sl.h, i));
 			});
 		for (int i = 0; i < n; i++) {
 			const int st = sl.h.status[i];
 			out_len[i] = sl.h.out_len[i];
 			if (in_used) in_used[i] = sl.h.in_used[i];
 			if (status) status[i] = st;
-			if (check) check[i] = wrap != B200Z_WRAP_RAW ? sl.h.check[i] : 0u;
+			if (check) check[i] = wrap != B200Z_WRAP_RAW || plan->kind == 2 ? sl.h.check[i] : 0u; // (LZW: the message's numbers)
 			if ((st & 0xFF) != B200Z_OK && first == B200Z_OK) {
 				first = st & 0xFF;
 				first_detail = (st >> 8) & 0xFF;
@@ -422,6 +440,13 @@ int b200z_pipeline_collect(b200z_pipeline *p, uint8_t *const *out, const int64_t
 	}
 	++p->tail;
 	if (first == B200Z_E_DATA && plan->kind == 1) set_error("%s", inflate_detail_msg(first_detail)); // the reference's exception message
+	else if (plan->kind == 2 && (first == B200Z_E_DATA || first == B200Z_E_INTERNAL)) {
+		for (int i = 0; i < n; i++)
+			if ((sl.h.status[i] & 0xFF) == first) {
+				set_error("%s", lzw_detail_msg(sl.h.status[i], sl.h.check[i]).c_str());
+				break;
+			}
+	}
 	else if (first != B200Z_OK) set_error("stream failed with status %d", first);
 	return first;
 }
@@ -448,6 +473,14 @@ int b200z_inflate_batch(const uint8_t *const *in, const int64_t *in_len, int32_t
 	if (rc) return rc;
 	const int32_t device = current_device();
 	return b200z_inflate_batch_multi(&device, 1, in, in_len, n, wrap, out, out_cap, out_len, in_used, check, status);
+}
+
+int b200z_lzw_batch(const uint8_t *const *in, const int64_t *in_len, int32_t n, uint8_t *const *out, const int64_t *out_cap,
+                    int64_t *out_len, int64_t *in_used, uint32_t *value, int32_t *status) {
+	int rc = ensure_init();
+	if (rc) return rc;
+	const int32_t device = current_device();
+	return b200z_lzw_batch_multi(&device, 1, in, in_len, n, out, out_cap, out_len, in_used, value, status);
 }
 
 // ---- one host thread, several GPUs ----------------------------------------------------------------------------------
@@ -497,6 +530,11 @@ int b200z_inflate_batch_multi(const int32_t *devices, int32_t n_devices, const u
                               uint8_t *const *out, const int64_t *out_cap, int64_t *out_len, int64_t *in_used, uint32_t *check,
                               int32_t *status) {
 	return multi_batch(1, devices, n_devices, in, in_len, n, 0, 0, wrap, 0, out, out_cap, out_len, in_used, check, status);
+}
+
+int b200z_lzw_batch_multi(const int32_t *devices, int32_t n_devices, const uint8_t *const *in, const int64_t *in_len, int32_t n,
+                          uint8_t *const *out, const int64_t *out_cap, int64_t *out_len, int64_t *in_used, uint32_t *value, int32_t *status) {
+	return multi_batch(2, devices, n_devices, in, in_len, n, 0, 0, B200Z_WRAP_RAW, 0, out, out_cap, out_len, in_used, value, status);
 }
 
 } // extern "C"

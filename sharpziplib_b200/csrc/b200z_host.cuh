@@ -32,5 +32,6 @@ int streams_down(const b200z_plan *plan, Staging &st, uint8_t *const *dst, cudaS
 
 void zlib_header(int level, uint8_t h[2], bool preset_dict = false);
 const char *inflate_detail_msg(int detail); // the reference's exception message for an inflate status detail
+std::string lzw_detail_msg(int32_t status, uint32_t value); // the reference's message for an LZW status and its numbers
 
 } // namespace b200z

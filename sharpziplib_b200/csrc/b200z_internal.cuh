@@ -150,7 +150,7 @@ struct b200z_plan {
 		for (cudaEvent_t e : ev) cudaEventDestroy(e);
 		if (ws.base) cudaFree(ws.base);
 	}
-	int kind = 0; // 0 deflate, 1 inflate
+	int kind = 0; // 0 deflate, 1 inflate, 2 LZW
 	int device = -1; // the device the plan's workspace lives on
 	int n = 0;
 	int level = 6, strategy = 0, wrap = 0, end_mode = 0;
@@ -221,4 +221,9 @@ int checksum_launch(int kind, const uint8_t *d_data, const int64_t *d_off, const
                     cudaStream_t s, bool dynamic);
 int checksum_tiles(const int64_t *len, int32_t n, std::vector<CkTile> &tiles, int kind, bool dynamic = false);
 int checksum_init_tables();
+// b200z_lzw.cu: LZW (.Z) plans; the run reports the numbers of a stream's error message in d_value
+int lzw_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, b200z_plan **out);
+int lzw_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status, uint32_t *d_value,
+                 int64_t *d_in_used, cudaStream_t s);
+int lzw_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s);
 } // namespace b200z
