@@ -56,14 +56,18 @@ int b200z_static_tables_import(const uint8_t *blob, int32_t len);
 int b200z_static_tables_broadcast(void *nccl_comm, int32_t root, int32_t rank, void *cuda_stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Checksums -- IChecksum (Checksum/IChecksum.cs), Crc32 (Checksum/Crc32.cs:47-171), Adler32 (Checksum/Adler32.cs:56-161).
- * `value` in/out is the checksum's Value over everything fed so far (Crc32.Reset -> 0, Adler32.Reset -> 1).
+ * Checksums -- IChecksum (Checksum/IChecksum.cs), Crc32 (Checksum/Crc32.cs:47-171), Adler32 (Checksum/Adler32.cs:56-161),
+ * BZip2Crc (Checksum/BZip2Crc.cs:43-170).
+ * `value` in/out is the checksum's Value over everything fed so far (Crc32.Reset -> 0, Adler32.Reset -> 1,
+ * BZip2Crc.Reset -> 0).  For BZip2Crc, Value is ~checkValue: an update from value v starts from the register ~v.
  * Host-buffer forms copy to the device and reduce there; _device forms take device pointers.
  * ------------------------------------------------------------------------------------------------------------- */
 int b200z_crc32(const uint8_t *buf, int64_t len, uint32_t *value);
+int b200z_bzip2crc(const uint8_t *buf, int64_t len, uint32_t *value);
 int b200z_adler32(const uint8_t *buf, int64_t len, uint32_t *value);
 /* n independent buffers resident on the device: buffer i is d_data[off[i] .. off[i]+len[i]); seeds/results in
- * d_value[i] (device).  kind: 0 = CRC32, 1 = Adler32.  off/len are host arrays.  Asynchronous on `stream`. */
+ * d_value[i] (device).  kind: 0 = CRC-32 (Crc32), 1 = Adler-32 (Adler32), 2 = CRC-32/BZIP2 (BZip2Crc); any other kind is
+ * B200Z_E_ARG.  off/len are host arrays.  Asynchronous on `stream`. */
 int b200z_checksum_batch_device(int kind, const uint8_t *d_data, const int64_t *off, const int64_t *len, int32_t n,
                                 uint32_t *d_value, void *cuda_stream);
 

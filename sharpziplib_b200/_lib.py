@@ -67,6 +67,7 @@ _SIGS = {
     "b200z_static_tables_export": (C.c_int, [C.c_void_p, C.c_int32]),
     "b200z_static_tables_import": (C.c_int, [C.c_void_p, C.c_int32]),
     "b200z_crc32": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint32)]),
+    "b200z_bzip2crc": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint32)]),
     "b200z_adler32": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint32)]),
     "b200z_checksum_batch_device": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200z_deflate_plan_create": (C.c_int, [C.c_int32, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),

@@ -1,5 +1,6 @@
-"""Crc32 / Adler32 -- mirrors of Checksum/Crc32.cs:47-171 and Checksum/Adler32.cs:56-161 (IChecksum: Reset, Value,
-Update).  The reduction runs on the GPU (b200z_checksum.cu); the object only keeps the running Value."""
+"""Crc32 / Adler32 / BZip2Crc -- mirrors of Checksum/Crc32.cs:47-171, Checksum/Adler32.cs:56-161 and
+Checksum/BZip2Crc.cs:43-170 (IChecksum: Reset, Value, Update).  The reduction runs on the GPU (b200z_checksum.cu); the
+object only keeps the running Value."""
 import ctypes as C
 
 import numpy as np
@@ -32,7 +33,8 @@ class _Checksum:
         return self._value
 
     def Update(self, data, offset=0, count=None):
-        """Update(int) takes the low 8 bits (Crc32.cs:100, Adler32.cs:96); Update(bytes/ArraySegment) the whole span."""
+        """Update(int) takes the low 8 bits (Crc32.cs:100, Adler32.cs:96, BZip2Crc.cs:99); Update(bytes/ArraySegment) the
+        whole span."""
         if isinstance(data, int):
             data = bytes([data & 0xFF])
         a = _as_u8(data, offset, count)
@@ -54,6 +56,12 @@ class Crc32(_Checksum):
     """CRC-32/ISO-HDLC: reflected 0xEDB88320, init/xorout 0xFFFFFFFF (Crc32.cs:50-59)."""
     _INIT = 0
     _fn = "b200z_crc32"
+
+
+class BZip2Crc(_Checksum):
+    """CRC-32/BZIP2: normal 0x04C11DB7, init/xorout 0xFFFFFFFF (BZip2Crc.cs:47-50).  Value is ~checkValue, so 0 after Reset."""
+    _INIT = 0
+    _fn = "b200z_bzip2crc"
 
 
 class Adler32(_Checksum):

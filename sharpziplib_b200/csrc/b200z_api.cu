@@ -504,11 +504,12 @@ int b200z_plan_pack(b200z_plan *plan, const uint8_t *d_out, const int64_t *d_out
 
 // ---- checksums ---------------------------------------------------------------------------------------
 int b200z_crc32(const uint8_t *buf, int64_t len, uint32_t *value) { return checksum_host(0, buf, len, value); }
+int b200z_bzip2crc(const uint8_t *buf, int64_t len, uint32_t *value) { return checksum_host(2, buf, len, value); }
 int b200z_adler32(const uint8_t *buf, int64_t len, uint32_t *value) { return checksum_host(1, buf, len, value); }
 
 int b200z_checksum_batch_device(int kind, const uint8_t *d_data, const int64_t *off, const int64_t *len, int32_t n,
                                 uint32_t *d_value, void *cuda_stream) {
-	if (kind < 0 || kind > 1 || n < 0 || (n > 0 && (!d_data || !off || !len || !d_value))) {
+	if (kind < 0 || kind > 2 || n < 0 || (n > 0 && (!d_data || !off || !len || !d_value))) {
 		set_error("bad arguments");
 		return B200Z_E_ARG;
 	}

@@ -212,10 +212,10 @@ int inflate_plan_resume_points(b200z_plan *p, int64_t *hdr_bit, int64_t *body_bi
 int inflate_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s);
 int inflate_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status,
                      uint32_t *d_check, int64_t *d_in_used, cudaStream_t s);
-// checksum over n device buffers (kind 0 = CRC32, 1 = Adler32); d_acc = 2 x uint64 scratch per stream;
+// checksum over n device buffers (kind 0 = CRC32, 1 = Adler32, 2 = CRC-32/BZIP2); d_acc = 2 x uint64 scratch per stream;
 // value in/out (device uint32), `fresh` != 0 starts from the Reset() value instead of reading d_value.
 // `dynamic`: the tiles were laid over capacities (checksum_tiles(..., dynamic = true)) and d_len holds the real lengths,
-// known only on the device: the kernel skips the tiles past them and works the multipliers out itself.
+// known only on the device: the kernel skips the tiles past them and works the multipliers out itself (kinds 0 and 1 only).
 int checksum_launch(int kind, const uint8_t *d_data, const int64_t *d_off, const int64_t *d_len, int32_t n,
                     const CkTile *d_tiles, int32_t n_tiles, unsigned long long *d_acc, uint32_t *d_value, int fresh,
                     cudaStream_t s, bool dynamic);
