@@ -100,18 +100,16 @@ struct __align__(16) InfShared {
 	uint16_t tok_val[32];
 };
 
-// Builds a root table of `R` bits + canonical side tables from code lengths (InflaterHuffmanTree.BuildTree :87-169
-// computes the same canonical assignment).  kind: 0 litlen, 1 dist, 2 meta (19 code-length symbols, 7-bit root, no
-// long codes possible).  Returns 0 or a detail code.  Executed by one lane.
-__device__ int build_table(const uint8_t *lens, int nsym, int R, uint32_t *tab, uint16_t *sorted, Canon *cn, int kind) {
-	uint32_t count[16], next[16];
-	for (int i = 0; i < 16; i++) count[i] = 0;
-	for (int s = 0; s < nsym; s++) count[lens[s]]++;
-	count[0] = 0;
-	int left = 1;
+// From the number of codes of every length 1..15: the Kraft check, the first canonical code of every length (next) and,
+// with a Canon, the bookkeeping for codes longer than the root table of `R` bits.  Returns 0 or D_OVERSUBSCRIBED.
+__device__ __forceinline__ int canon_setup(const uint32_t *count, uint32_t *next, Canon *cn, int R) {
+	int left = 1, err = 0;
 	for (int L = 1; L <= 15; L++) {
 		left = (left << 1) - (int)count[L];
-		if (left < 0) return D_OVERSUBSCRIBED;
+		if (left < 0) {
+			err = D_OVERSUBSCRIBED;
+			break;
+		}
 	}
 	uint32_t code = 0, off = 0;
 	for (int L = 1; L <= 15; L++) {
@@ -124,6 +122,18 @@ __device__ int build_table(const uint8_t *lens, int nsym, int R, uint32_t *tab, 
 		if (L > R) off += count[L];
 		code = (code + count[L]) << 1;
 	}
+	return err;
+}
+
+// Builds a root table of `R` bits + canonical side tables from code lengths (InflaterHuffmanTree.BuildTree :87-169
+// computes the same canonical assignment).  kind: 0 litlen, 1 dist, 2 meta (19 code-length symbols, 7-bit root, no
+// long codes possible).  Returns 0 or a detail code.  Executed by one lane.
+__device__ int build_table(const uint8_t *lens, int nsym, int R, uint32_t *tab, uint16_t *sorted, Canon *cn, int kind) {
+	uint32_t count[16], next[16];
+	for (int i = 0; i < 16; i++) count[i] = 0;
+	for (int s = 0; s < nsym; s++) count[lens[s]]++;
+	const int d = canon_setup(count, next, cn, R);
+	if (d) return d;
 	const int size = 1 << R;
 	for (int i = 0; i < size; i++) tab[i] = 0;
 	for (int s = 0; s < nsym; s++) {
@@ -142,6 +152,16 @@ __device__ int build_table(const uint8_t *lens, int nsym, int R, uint32_t *tab, 
 	return 0;
 }
 
+// word wi of a stream of nbytes bytes (nwords words, the last one masked to the stream's bytes); 0 past the end
+__device__ __forceinline__ uint32_t ld_stream_word(const uint32_t *gwords, uint32_t wi, uint32_t nwords, uint32_t nbytes) {
+	uint32_t w = 0;
+	if (wi < nwords) {
+		w = __ldg(gwords + wi);
+		if (wi == nwords - 1 && (nbytes & 3)) w &= (1u << (8 * (nbytes & 3))) - 1u;
+	}
+	return w;
+}
+
 struct BitReader {
 	const uint32_t *words; // 4-byte aligned stream base
 	uint64_t bb;
@@ -150,15 +170,28 @@ struct BitReader {
 	uint32_t nwords; // words that hold stream bytes (the last one is masked)
 	uint32_t nbytes;
 	uint64_t consumed; // bits handed out so far
+	// a reader of a stream of nbytes bytes at bit position bitpos
+	static __device__ __forceinline__ BitReader at(const uint32_t *words, uint32_t nbytes, uint64_t bitpos) {
+		BitReader br;
+		br.words = words;
+		br.nbytes = nbytes;
+		br.nwords = (nbytes + 3) >> 2;
+		br.consumed = bitpos;
+		br.widx = (uint32_t)(bitpos >> 5);
+		br.bb = 0;
+		br.bc = 0;
+		const uint32_t sk = (uint32_t)(bitpos & 31);
+		if (sk) {
+			br.refill();
+			br.bb >>= sk;
+			br.bc -= sk;
+		}
+		return br;
+	}
 	__device__ __forceinline__ void refill() {
 		if (bc <= 32) {
-			uint32_t w = 0;
-			if (widx < nwords) {
-				w = __ldg(words + widx);
-				if (widx == nwords - 1 && (nbytes & 3)) w &= (1u << (8 * (nbytes & 3))) - 1u;
-			}
+			bb |= (uint64_t)ld_stream_word(words, widx, nwords, nbytes) << bc;
 			++widx;
-			bb |= (uint64_t)w << bc;
 			bc += 32;
 		}
 	}
@@ -177,27 +210,107 @@ struct BitReader {
 	__device__ __forceinline__ bool overrun() const { return consumed > 8ull * nbytes; }
 };
 
-// decodes one symbol of a tree with long-code fallback; returns the entry (nb already dropped) or 0 when invalid
-__device__ __forceinline__ uint32_t decode_sym(BitReader &br, const uint32_t *tab, int R, const uint16_t *sorted,
-                                               const Canon &cn, int kind) {
-	br.refill();
-	uint32_t e = tab[(uint32_t)br.bb & ((1u << R) - 1u)];
-	const uint32_t k = (e >> 4) & 15;
-	if (k != K_LONG) {
-		if (k != K_INVALID) br.drop(e & 15);
-		return e;
-	}
-	const uint32_t x = __brev((uint32_t)br.bb) >> 17; // next 15 stream bits, first bit most significant
+// the entry of a code longer than the root table of `R` bits at `v` (the next 32 stream bits); 0 (K_INVALID) when there is none
+__device__ uint32_t long_code(uint32_t v, const uint16_t *sorted, const Canon &cn, int R, int kind) {
+	const uint32_t x = __brev(v) >> 17; // next 15 stream bits, first bit most significant
 	for (int L = R + 1; L <= 15; L++) {
 		const uint32_t c = x >> (15 - L);
 		const uint32_t idx = c - cn.first[L];
 		if (idx < cn.count[L]) {
 			const uint32_t s = sorted[cn.offs[L] + idx];
-			br.drop(L);
-			return kind == 0 ? litlen_entry(s, L) : dist_entry(s, L);
+			return kind == 0 ? litlen_entry(s, (uint32_t)L) : dist_entry(s, (uint32_t)L);
 		}
 	}
-	return 0;
+	return 0; // K_INVALID, nb = 0
+}
+
+// the code lengths of a static block (InflaterHuffmanTree.cs:34-70): lens[0 .. 288) literal/length, lens[288 .. 320)
+// distance; set by the threads first, first + stride, ...  (Range by range: for k_inflate's one thread these loops are
+// constant stores, where a select per index cost it registers and spills.)
+__device__ __forceinline__ void static_lens(uint8_t *lens, int first, int stride) {
+	for (int i = first; i < 144; i += stride) lens[i] = 8;
+	for (int i = 144 + first; i < 256; i += stride) lens[i] = 9;
+	for (int i = 256 + first; i < 280; i += stride) lens[i] = 7;
+	for (int i = 280 + first; i < 288; i += stride) lens[i] = 8;
+	for (int i = 288 + first; i < 320; i += stride) lens[i] = 5;
+}
+
+struct BlockHeader {
+	int status, detail, btype, last, nlit, ndist;
+	uint32_t stored_len;
+};
+
+// Reads a block header from br's position up to the block's first symbol (Inflater.Decode :459-512 and, for a dynamic block,
+// InflaterDynHeader.CreateStateMachine :42-120).  A dynamic block's code lengths are left in sh.lens[0 .. nlit + ndist), its
+// code tables are the caller's to build.  Executed by one thread.
+__device__ BlockHeader read_block_header(BitReader &br, InfShared &sh) {
+	BlockHeader h = {B200Z_OK, 0, 0, 0, 288, 32, 0};
+	const uint32_t hdr = br.get(3);
+	if (br.overrun()) {
+		h.status = B200Z_E_NEED_INPUT;
+	} else {
+		h.last = (int)(hdr & 1u);
+		h.btype = (int)(hdr >> 1);
+		if (h.btype == 0) { // SkipToByteBoundary, LEN, NLEN (Inflater.cs:509)
+			br.drop(br.bc & 7);
+			const uint32_t len = br.get(16);
+			const uint32_t nlen = br.get(16);
+			if (br.overrun()) h.status = B200Z_E_NEED_INPUT;
+			else if (nlen != (len ^ 0xFFFFu)) { h.status = B200Z_E_DATA; h.detail = D_STORED_LEN; }
+			h.stored_len = len;
+		} else if (h.btype == 2) {
+			h.nlit = (int)br.get(5) + 257;
+			h.ndist = (int)br.get(5) + 1;
+			const int nmeta = (int)br.get(4) + 4;
+			if (h.nlit > 286 || h.ndist > 30) { h.status = B200Z_E_DATA; h.detail = D_HDR_RANGE; }
+			else {
+				for (int i = 0; i < 19; i++) sh.lens[i] = 0;
+				for (int i = 0; i < nmeta; i++) sh.lens[c_meta_order[i]] = (uint8_t)br.get(3);
+				const int d = build_table(sh.lens, 19, 7, sh.meta, nullptr, nullptr, 2);
+				if (d) { h.status = B200Z_E_DATA; h.detail = d; }
+				const int total = h.nlit + h.ndist;
+				int idx = 0;
+				while (h.status == B200Z_OK && idx < total) {
+					br.refill();
+					const uint32_t e = sh.meta[br.peek(7)];
+					if (((e >> 4) & 15) == K_INVALID) { h.status = B200Z_E_DATA; h.detail = D_CODELEN0; break; }
+					br.drop(e & 15);
+					const int sym = (int)(e >> 16);
+					if (sym < 16) {
+						sh.lens[idx++] = (uint8_t)sym;
+					} else {
+						int rep;
+						uint8_t v = 0;
+						if (sym == 16) {
+							if (idx == 0) { h.status = B200Z_E_DATA; h.detail = D_HDR_REPEAT0; break; }
+							v = sh.lens[idx - 1];
+							rep = 3 + (int)br.get(2);
+						} else if (sym == 17) rep = 3 + (int)br.get(3);
+						else rep = 11 + (int)br.get(7);
+						if (idx + rep > total) { h.status = B200Z_E_DATA; h.detail = D_HDR_OVERRUN; break; }
+						while (rep-- > 0) sh.lens[idx++] = v;
+					}
+					if (br.overrun()) { h.status = B200Z_E_NEED_INPUT; break; }
+				}
+				if (h.status == B200Z_OK && br.overrun()) h.status = B200Z_E_NEED_INPUT;
+				if (h.status == B200Z_OK && sh.lens[256] == 0) { h.status = B200Z_E_DATA; h.detail = D_HDR_NO_EOB; }
+			}
+		} else if (h.btype == 3) {
+			h.status = B200Z_E_DATA;
+			h.detail = D_BLOCK_TYPE;
+		}
+	}
+	// an error diagnosed from bits past the end of the input is "needs more input", not corrupt data
+	if (h.status != B200Z_OK && br.overrun()) { h.status = B200Z_E_NEED_INPUT; h.detail = 0; }
+	return h;
+}
+
+// A stream entered in mid-block (b200z_inflate_plan_set_resume) reads a copy of the block's header and goes on decoding at
+// bit `skip` (0: not entered in mid-block).  Only a Huffman block can be entered in the middle, and not inside its own header.
+__device__ __forceinline__ void enter_mid_block(BlockHeader &h, BitReader &br, uint64_t skip) {
+	if (h.status != B200Z_OK || !skip) return;
+	if (h.btype == 0 || br.consumed > skip) { h.status = B200Z_E_ARG; h.detail = 0; }
+	else br.consumed = skip;
 }
 
 constexpr int kSubBits = 512;                 // input bits per lane per round
@@ -207,6 +320,11 @@ constexpr int kInWords = kRoundWords + 8;        // + slack for the last symbol'
 // every peek).  One pad word per 16 moves lane l to 17 l.
 __device__ __forceinline__ uint32_t in_slot(uint32_t i) { return i + (i >> 4); }
 constexpr int kInSlots = kInWords + kInWords / 16 + 1;
+// words[in_slot(i)] = stream word w0 + i for i < count, taken by the threads first, first + stride, ...
+__device__ __forceinline__ void stage_words(uint32_t *words, const uint32_t *gwords, uint32_t w0, int count, uint32_t nwords,
+                                            uint32_t nbytes, int first, int stride) {
+	for (int i = first; i < count; i += stride) words[in_slot((uint32_t)i)] = ld_stream_word(gwords, w0 + (uint32_t)i, nwords, nbytes);
+}
 constexpr int kLaneOutCap = 512;                 // output bytes a lane may produce per round
 constexpr int kRing = 65536;                     // output ring: 32 KiB of history + the two rounds the consumer warps hold (2 x 32 x kLaneOutCap)
 constexpr int kMList = 32;                       // back-references a lane may record per round
@@ -239,22 +357,10 @@ __device__ __forceinline__ uint32_t peek32(const uint32_t *w, uint32_t pos) {
 // decodes one symbol of a tree at `v` (the next 32 stream bits); returns the entry and the code length in nb
 __device__ __forceinline__ uint32_t lane_decode_sym(uint32_t v, const uint32_t *tab, int R, const uint16_t *sorted,
                                                     const Canon &cn, int kind, uint32_t &nb) {
-	const uint32_t e = tab[v & ((1u << R) - 1u)];
-	const uint32_t k = (e >> 4) & 15;
+	uint32_t e = tab[v & ((1u << R) - 1u)];
+	if (((e >> 4) & 15) == K_LONG) e = long_code(v, sorted, cn, R, kind);
 	nb = e & 15;
-	if (k != K_LONG) return e;
-	const uint32_t x = __brev(v) >> 17; // next 15 stream bits, first bit most significant
-	for (int L = R + 1; L <= 15; L++) {
-		const uint32_t c = x >> (15 - L);
-		const uint32_t idx = c - cn.first[L];
-		if (idx < cn.count[L]) {
-			const uint32_t s = sorted[cn.offs[L] + idx];
-			nb = (uint32_t)L;
-			return kind == 0 ? litlen_entry(s, L) : dist_entry(s, L);
-		}
-	}
-	nb = 0;
-	return 0;
+	return e;
 }
 
 // Per-lane decode state of one span (the symbols that START in [entry, limit), relative bit positions).
@@ -377,15 +483,8 @@ __global__ void __launch_bounds__(kInfThreads)
 	const uint64_t cap = (uint64_t)out_cap[stream];
 	const uint32_t *gwords = reinterpret_cast<const uint32_t *>(in + in_off[stream]);
 
-	BitReader br; // warp A lane 0's header reader (global memory)
-	br.words = gwords;
-	br.nbytes = (uint32_t)in_len[stream];
-	br.nwords = (br.nbytes + 3) >> 2;
-	br.bb = 0;
-	br.bc = 0;
-	br.widx = 0;
-	br.consumed = 0;
-	const uint64_t total_bits = 8ull * br.nbytes;
+	const uint32_t nbytes = (uint32_t)in_len[stream], nwords = (nbytes + 3) >> 2;
+	const uint64_t total_bits = 8ull * nbytes;
 
 	for (int i = threadIdx.x; i < kRing / 16; i += kInfThreads) reinterpret_cast<uint4 *>(S.ring)[i] = make_uint4(0, 0, 0, 0); // fresh window = zeros
 	if (threadIdx.x == 0) {
@@ -433,7 +532,7 @@ __global__ void __launch_bounds__(kInfThreads)
 					if (!b_busy) {
 						// ---- stored block: OutputWindow.CopyStored (:100-122); B is idle, so the ring and dst are ours
 						const uint64_t ipos = bitpos >> 3;
-						const uint64_t avail = ipos <= br.nbytes ? br.nbytes - ipos : 0;
+						const uint64_t avail = ipos <= nbytes ? nbytes - ipos : 0;
 						if (stored_len > avail) st = B200Z_E_NEED_INPUT;
 						else if (opos + stored_len > cap) st = B200Z_E_NOMEM;
 						if (st == B200Z_OK) {
@@ -462,103 +561,31 @@ __global__ void __launch_bounds__(kInfThreads)
 						}
 						uint64_t hend = bitpos;
 						if (lane == 0) {
-							// re-seat the header reader at the true bit position
-							br.consumed = bitpos;
-							br.widx = (uint32_t)(bitpos >> 5);
-							br.bb = 0;
-							br.bc = 0;
-							const uint32_t sk = (uint32_t)(bitpos & 31);
-							if (sk) {
-								br.refill();
-								br.bb >>= sk;
-								br.bc -= sk;
-							}
 							if (last) {
 								btype = -1; // Inflater.cs:443-449: raw mode stops right after the final block
 							} else {
-								const uint32_t hdr = br.get(3);
-								if (br.overrun()) {
-									st = B200Z_E_NEED_INPUT;
-								} else {
-									last = (hdr & 1) != 0;
-									btype = (int)(hdr >> 1);
-									InfShared &sh = S.sh[ntab];
-									if (btype == 0) {
-										// SkipToByteBoundary, LEN, NLEN (:509)
-										br.drop(br.bc & 7);
-										const uint32_t len = br.get(16);
-										const uint32_t nlen = br.get(16);
-										if (br.overrun()) st = B200Z_E_NEED_INPUT;
-										else if (nlen != (len ^ 0xFFFFu)) { st = B200Z_E_DATA; detail = D_STORED_LEN; }
-										stored_len = len;
-									} else if (btype == 1) {
-										if (static_in != ntab) {
-											for (int i = 0; i < 144; i++) sh.lens[i] = 8;
-											for (int i = 144; i < 256; i++) sh.lens[i] = 9;
-											for (int i = 256; i < 280; i++) sh.lens[i] = 7;
-											for (int i = 280; i < 288; i++) sh.lens[i] = 8;
-											build_table(sh.lens, 288, kLitRoot, sh.lit, sh.lit_sorted, &sh.lit_c, 0);
-											for (int i = 0; i < 32; i++) sh.lens[i] = 5;
-											build_table(sh.lens, 32, kDistRoot, sh.dist, sh.dist_sorted, &sh.dist_c, 1);
-											static_in = ntab;
-										}
-									} else if (btype == 2) {
-										if (static_in == ntab) static_in = -1;
-										// InflaterDynHeader.CreateStateMachine (:42-120)
-										const int nlit = (int)br.get(5) + 257, ndist = (int)br.get(5) + 1, nmeta = (int)br.get(4) + 4;
-										if (nlit > 286 || ndist > 30) { st = B200Z_E_DATA; detail = D_HDR_RANGE; }
-										else {
-											for (int i = 0; i < 19; i++) sh.lens[i] = 0;
-											for (int i = 0; i < nmeta; i++) sh.lens[c_meta_order[i]] = (uint8_t)br.get(3);
-											int d = build_table(sh.lens, 19, 7, sh.meta, nullptr, nullptr, 2);
-											if (d) { st = B200Z_E_DATA; detail = d; }
-											const int total = nlit + ndist;
-											int idx = 0;
-											while (st == B200Z_OK && idx < total) {
-												br.refill();
-												const uint32_t e = sh.meta[br.peek(7)];
-												if (((e >> 4) & 15) == K_INVALID) { st = B200Z_E_DATA; detail = D_CODELEN0; break; }
-												br.drop(e & 15);
-												const int sym = (int)(e >> 16);
-												if (sym < 16) {
-													sh.lens[idx++] = (uint8_t)sym;
-												} else {
-													int rep;
-													uint8_t v = 0;
-													if (sym == 16) {
-														if (idx == 0) { st = B200Z_E_DATA; detail = D_HDR_REPEAT0; break; }
-														v = sh.lens[idx - 1];
-														rep = 3 + (int)br.get(2);
-													} else if (sym == 17) rep = 3 + (int)br.get(3);
-													else rep = 11 + (int)br.get(7);
-													if (idx + rep > total) { st = B200Z_E_DATA; detail = D_HDR_OVERRUN; break; }
-													while (rep-- > 0) sh.lens[idx++] = v;
-												}
-												if (br.overrun()) { st = B200Z_E_NEED_INPUT; break; }
-											}
-											if (st == B200Z_OK && br.overrun()) st = B200Z_E_NEED_INPUT;
-											if (st == B200Z_OK && sh.lens[256] == 0) { st = B200Z_E_DATA; detail = D_HDR_NO_EOB; }
-											if (st == B200Z_OK) {
-												uint8_t dl[32];
-												for (int i = 0; i < ndist; i++) dl[i] = sh.lens[nlit + i];
-												d = build_table(sh.lens, nlit, kLitRoot, sh.lit, sh.lit_sorted, &sh.lit_c, 0);
-												if (!d) d = build_table(dl, ndist, kDistRoot, sh.dist, sh.dist_sorted, &sh.dist_c, 1);
-												if (d) { st = B200Z_E_DATA; detail = d; }
-											}
-										}
-									} else {
-										st = B200Z_E_DATA;
-										detail = D_BLOCK_TYPE;
-									}
+								BitReader br = BitReader::at(gwords, nbytes, bitpos);
+								InfShared &sh = S.sh[ntab];
+								BlockHeader h = read_block_header(br, sh);
+								if (h.status == B200Z_OK && h.btype == 1 && static_in != ntab) {
+									static_lens(sh.lens, 0, 1);
+									build_table(sh.lens, 288, kLitRoot, sh.lit, sh.lit_sorted, &sh.lit_c, 0);
+									build_table(sh.lens + 288, 32, kDistRoot, sh.dist, sh.dist_sorted, &sh.dist_c, 1);
+									static_in = ntab;
+								} else if (h.status == B200Z_OK && h.btype == 2) {
+									if (static_in == ntab) static_in = -1;
+									int d = build_table(sh.lens, h.nlit, kLitRoot, sh.lit, sh.lit_sorted, &sh.lit_c, 0);
+									if (!d) d = build_table(sh.lens + h.nlit, h.ndist, kDistRoot, sh.dist, sh.dist_sorted, &sh.dist_c, 1);
+									if (d) { h.status = B200Z_E_DATA; h.detail = d; }
 								}
-							}
-							// an error diagnosed from bits past the end of the input is "needs more input", not corrupt data
-							if (st != B200Z_OK && br.overrun()) { st = B200Z_E_NEED_INPUT; detail = 0; }
-							hend = br.consumed;
-							// only a Huffman block can be entered in the middle, and not inside its own header
-							if (st == B200Z_OK && first_hdr && skip) {
-								if (btype == 0 || hend > skip) { st = B200Z_E_ARG; detail = 0; }
-								else br.consumed = skip;
+								hend = br.consumed;
+								if (first_hdr) enter_mid_block(h, br, skip);
+								st = h.status;
+								detail = h.detail;
+								btype = h.btype;
+								last = h.last != 0;
+								stored_len = h.stored_len;
+								bitpos = br.consumed;
 							}
 						}
 						first_hdr = false;
@@ -567,7 +594,7 @@ __global__ void __launch_bounds__(kInfThreads)
 						btype = __shfl_sync(0xffffffffu, btype, 0);
 						last = __shfl_sync(0xffffffffu, (int)last, 0) != 0;
 						static_in = __shfl_sync(0xffffffffu, static_in, 0);
-						bitpos = __shfl_sync(0xffffffffu, (unsigned long long)br.consumed, 0);
+						bitpos = __shfl_sync(0xffffffffu, (unsigned long long)bitpos, 0);
 						stored_len = __shfl_sync(0xffffffffu, stored_len, 0);
 						__syncwarp();
 						if (st != B200Z_OK || btype == -1) {
@@ -585,15 +612,7 @@ __global__ void __launch_bounds__(kInfThreads)
 						uint32_t *words = S.in[cur];
 						const InfShared &sh = S.sh[tab];
 						const uint32_t w0 = (uint32_t)(bitpos >> 5);
-						for (int i = lane; i < kInWords; i += 32) {
-							const uint32_t wi = w0 + (uint32_t)i;
-							uint32_t v = 0;
-							if (wi < br.nwords) {
-								v = __ldg(gwords + wi);
-								if (wi == br.nwords - 1 && (br.nbytes & 3)) v &= (1u << (8 * (br.nbytes & 3))) - 1u;
-							}
-							words[in_slot((uint32_t)i)] = v;
-						}
+						stage_words(words, gwords, w0, kInWords, nwords, nbytes, lane, 32);
 						__syncwarp();
 						const uint32_t r0 = (uint32_t)(bitpos & 31);
 						const uint64_t remain = total_bits - ((uint64_t)w0 << 5);
@@ -795,7 +814,7 @@ __global__ void __launch_bounds__(kInfThreads)
 		out_len[stream] = (int64_t)opos;
 		if (in_used) {
 			uint64_t used = (bitpos + 7) >> 3; // n - RemainingInput (trap T14)
-			if (used > br.nbytes) used = br.nbytes;
+			if (used > nbytes) used = nbytes;
 			in_used[stream] = (int64_t)used;
 		}
 		// (a round that did not fit the output leaves bitpos / opos at its first symbol, like one that ran out of input)

@@ -85,15 +85,6 @@ struct PCounters {
 // ---------------------------------------------------------------------------------------------------------
 // finder
 // ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t ld_stream_word(const uint32_t *gwords, uint32_t wi, uint32_t nwords, uint32_t nbytes) {
-	uint32_t w = 0;
-	if (wi < nwords) {
-		w = __ldg(gwords + wi);
-		if (wi == nwords - 1 && (nbytes & 3)) w &= (1u << (8 * (nbytes & 3))) - 1u;
-	}
-	return w;
-}
-
 // Stages 1 and 2.  32 bit offsets at a time: the fixed header fields as bit-parallel masks over funnel-shifted words; the
 // positions that pass (11 %) are compacted per warp so that every lane has one to test, then the Kraft sum of the
 // code-length code (a complete code: sum of 2^(7-len) = 128) through a table of four lengths at a time.
@@ -198,20 +189,7 @@ __global__ void __launch_bounds__(128)
 		const unsigned long long e = fs_list[i];
 		const uint32_t stream = (uint32_t)(e >> 40);
 		const uint64_t pos = e & ((1ull << 40) - 1ull);
-		BitReader br;
-		br.words = reinterpret_cast<const uint32_t *>(in + in_off[stream]);
-		br.nbytes = (uint32_t)in_len[stream];
-		br.nwords = (br.nbytes + 3) >> 2;
-		br.consumed = pos;
-		br.widx = (uint32_t)(pos >> 5);
-		br.bb = 0;
-		br.bc = 0;
-		const uint32_t sk = (uint32_t)(pos & 31);
-		if (sk) {
-			br.refill();
-			br.bb >>= sk;
-			br.bc -= sk;
-		}
+		BitReader br = BitReader::at(reinterpret_cast<const uint32_t *>(in + in_off[stream]), (uint32_t)in_len[stream], pos);
 		br.get(3);
 		const int nlit = (int)br.get(5) + 257, ndist = (int)br.get(5) + 1, nmeta = (int)br.get(4) + 4;
 		// the code-length code's lengths, 3 bits each, kept in one word per ten symbols
@@ -342,25 +320,8 @@ __device__ int build_tables_cta(InfShared &sh, TabScratch &ts, int nlit, int ndi
 	}
 	__syncthreads();
 	if (tid < 2) {
-		const int k = tid, R = k ? kDistRoot : kLitRoot;
-		Canon &cn = k ? sh.dist_c : sh.lit_c;
-		int left = 1;
-		for (int L = 1; L <= 15; L++) {
-			left = (left << 1) - (int)ts.cnt[k][L];
-			if (left < 0) {
-				ts.err = D_OVERSUBSCRIBED;
-				break;
-			}
-		}
-		uint32_t code = 0, off = 0;
-		for (int L = 1; L <= 15; L++) {
-			ts.nxt[k][L] = code;
-			cn.first[L] = (uint16_t)code;
-			cn.count[L] = (uint16_t)ts.cnt[k][L];
-			cn.offs[L] = (uint16_t)off;
-			if (L > R) off += ts.cnt[k][L];
-			code = (code + ts.cnt[k][L]) << 1;
-		}
+		const int d = canon_setup(ts.cnt[tid], ts.nxt[tid], tid ? &sh.dist_c : &sh.lit_c, tid ? kDistRoot : kLitRoot);
+		if (d) ts.err = d;
 	}
 	__syncthreads();
 	const int err = ts.err;
@@ -400,10 +361,6 @@ __device__ int build_tables_cta(InfShared &sh, TabScratch &ts, int nlit, int ndi
 	return 0;
 }
 
-__device__ __forceinline__ void static_lens(uint8_t *lens) { // InflaterHuffmanTree.cs:34-70
-	for (int i = threadIdx.x; i < 320; i += blockDim.x) lens[i] = (uint8_t)(i < 144 ? 8 : (i < 256 ? 9 : (i < 280 ? 7 : (i < 288 ? 8 : 5))));
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // span decode without per-lane caps.  MODE 0 counts; MODE 1 stores literals at out[o0 + o] and back-references at
 // ml[nm] (output positions relative to the stream).
@@ -412,18 +369,6 @@ __device__ __forceinline__ void static_lens(uint8_t *lens) { // InflaterHuffmanT
 // lane always holds a literal and some lane a back-reference, so both paths would be paid for anyway.  Every lane peeks
 // twice (the literal/length code, and what follows its extra bits -- the distance code if it was a length) and selects.
 // Codes longer than the root tables, end of block and the error cases leave through rare branches.
-__device__ uint32_t long_code(uint32_t v, const uint16_t *sorted, const Canon &cn, int R, int kind) {
-	const uint32_t x = __brev(v) >> 17; // next 15 stream bits, first bit most significant
-	for (int L = R + 1; L <= 15; L++) {
-		const uint32_t c = x >> (15 - L);
-		const uint32_t idx = c - cn.first[L];
-		if (idx < cn.count[L]) {
-			const uint32_t s = sorted[cn.offs[L] + idx];
-			return kind == 0 ? litlen_entry(s, (uint32_t)L) : dist_entry(s, (uint32_t)L);
-		}
-	}
-	return 0; // K_INVALID, nb = 0
-}
 
 // A lane's decode state: the bit position and, in registers, the next 33..64 bits of the stream from there (refilled 32 bits
 // at a time from the staged words), so that a literal costs one table lookup and a few shifts -- no shared-memory round
@@ -564,11 +509,6 @@ struct __align__(16) Dec1Shared {
 	uint32_t nlive[2];
 };
 
-__device__ __forceinline__ void stage_round(uint32_t *words, const uint32_t *gwords, uint32_t w0, uint32_t nwords, uint32_t nbytes) {
-	for (int i = threadIdx.x; i < kP1InWords; i += blockDim.x)
-		words[in_slot((uint32_t)i)] = ld_stream_word(gwords, w0 + (uint32_t)i, nwords, nbytes);
-}
-
 __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per SM (the header parse would take 64)
     k_dec1(const uint8_t *__restrict__ in, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len, PSeg *__restrict__ segs,
            const uint32_t *__restrict__ seg_list, PCounters *__restrict__ ctr, const uint32_t *__restrict__ win_base,
@@ -615,97 +555,19 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
 			rs_out = opos;
 			// ---- block header (thread 0) -----------------------------------------------------------------------
 			if (tid == 0) {
-				BitReader br;
-				br.words = gwords;
-				br.nbytes = nbytes;
-				br.nwords = nwords;
-				br.consumed = bitpos;
-				br.widx = (uint32_t)(bitpos >> 5);
-				br.bb = 0;
-				br.bc = 0;
-				const uint32_t sk = (uint32_t)(bitpos & 31);
-				if (sk) {
-					br.refill();
-					br.bb >>= sk;
-					br.bc -= sk;
-				}
-				int hst = B200Z_OK, hdet = 0, btype = 0, hlast = 0, nlit = 288, ndist = 32;
-				uint32_t stored_len = 0;
-				const uint32_t hdr = br.get(3);
-				if (br.overrun()) {
-					hst = B200Z_E_NEED_INPUT;
-				} else {
-					hlast = (int)(hdr & 1u);
-					btype = (int)(hdr >> 1);
-					InfShared &sh = S.sh;
-					if (btype == 0) { // SkipToByteBoundary, LEN, NLEN (Inflater.cs:509)
-						br.drop(br.bc & 7);
-						const uint32_t len = br.get(16);
-						const uint32_t nlen = br.get(16);
-						if (br.overrun()) hst = B200Z_E_NEED_INPUT;
-						else if (nlen != (len ^ 0xFFFFu)) { hst = B200Z_E_DATA; hdet = D_STORED_LEN; }
-						stored_len = len;
-					} else if (btype == 2) { // InflaterDynHeader.CreateStateMachine (:42-120)
-						nlit = (int)br.get(5) + 257;
-						ndist = (int)br.get(5) + 1;
-						const int nmeta = (int)br.get(4) + 4;
-						if (nlit > 286 || ndist > 30) { hst = B200Z_E_DATA; hdet = D_HDR_RANGE; }
-						else {
-							for (int i = 0; i < 19; i++) sh.lens[i] = 0;
-							for (int i = 0; i < nmeta; i++) sh.lens[c_meta_order[i]] = (uint8_t)br.get(3);
-							const int d = build_table(sh.lens, 19, 7, sh.meta, nullptr, nullptr, 2);
-							if (d) { hst = B200Z_E_DATA; hdet = d; }
-							const int total = nlit + ndist;
-							int idx = 0;
-							while (hst == B200Z_OK && idx < total) {
-								br.refill();
-								const uint32_t e = sh.meta[br.peek(7)];
-								if (((e >> 4) & 15) == K_INVALID) { hst = B200Z_E_DATA; hdet = D_CODELEN0; break; }
-								br.drop(e & 15);
-								const int sym = (int)(e >> 16);
-								if (sym < 16) {
-									sh.lens[idx++] = (uint8_t)sym;
-								} else {
-									int rep;
-									uint8_t v = 0;
-									if (sym == 16) {
-										if (idx == 0) { hst = B200Z_E_DATA; hdet = D_HDR_REPEAT0; break; }
-										v = sh.lens[idx - 1];
-										rep = 3 + (int)br.get(2);
-									} else if (sym == 17) rep = 3 + (int)br.get(3);
-									else rep = 11 + (int)br.get(7);
-									if (idx + rep > total) { hst = B200Z_E_DATA; hdet = D_HDR_OVERRUN; break; }
-									while (rep-- > 0) sh.lens[idx++] = v;
-								}
-								if (br.overrun()) { hst = B200Z_E_NEED_INPUT; break; }
-							}
-							if (hst == B200Z_OK && br.overrun()) hst = B200Z_E_NEED_INPUT;
-							if (hst == B200Z_OK && sh.lens[256] == 0) { hst = B200Z_E_DATA; hdet = D_HDR_NO_EOB; }
-						}
-					} else if (btype == 3) {
-						hst = B200Z_E_DATA;
-						hdet = D_BLOCK_TYPE;
-					}
-				}
-				// an error diagnosed from bits past the end of the input is "needs more input", not corrupt data
-				if (hst != B200Z_OK && br.overrun()) { hst = B200Z_E_NEED_INPUT; hdet = 0; }
-				const uint64_t hend = br.consumed;
-				S.h_body = (hst == B200Z_OK && (btype == 1 || btype == 2)) ? hend : bitpos;
-				// the stream-start segment (slot == stream) of a stream entered in mid-block: the header is a copy, decoding goes on at
-				// skip_bit; only a Huffman block can be entered there, and not inside its own header
-				if (hst == B200Z_OK && !blocks_done && slot == stream && skip_bit && skip_bit[stream]) {
-					const uint64_t skip = (uint64_t)skip_bit[stream];
-					if (btype == 0 || hend > skip) { hst = B200Z_E_ARG; hdet = 0; }
-					else br.consumed = skip;
-				}
-				S.h_st = hst;
-				S.h_detail = hdet;
-				S.h_btype = btype;
-				S.h_last = hlast;
-				S.h_nlit = nlit;
-				S.h_ndist = ndist;
+				BitReader br = BitReader::at(gwords, nbytes, bitpos);
+				BlockHeader h = read_block_header(br, S.sh);
+				S.h_body = (h.status == B200Z_OK && (h.btype == 1 || h.btype == 2)) ? br.consumed : bitpos;
+				// the stream-start segment (slot == stream) of a stream entered in mid-block: the header is a copy
+				if (!blocks_done && slot == stream && skip_bit) enter_mid_block(h, br, (uint64_t)skip_bit[stream]);
+				S.h_st = h.status;
+				S.h_detail = h.detail;
+				S.h_btype = h.btype;
+				S.h_last = h.last;
+				S.h_nlit = h.nlit;
+				S.h_ndist = h.ndist;
 				S.h_bitpos = br.consumed;
-				S.h_stored_len = stored_len;
+				S.h_stored_len = h.stored_len;
 			}
 			__syncthreads();
 			st = S.h_st;
@@ -751,7 +613,7 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
 			int nlit = S.h_nlit, ndist = S.h_ndist;
 			if (btype == 1) {
 				__syncthreads();
-				static_lens(S.sh.lens);
+				static_lens(S.sh.lens, tid, (int)blockDim.x);
 				nlit = 288;
 				ndist = 32;
 				__syncthreads();
@@ -789,7 +651,7 @@ __global__ void __launch_bounds__(kP1Threads, 10) // 48 registers: ten CTAs per 
 					S.nlive[0] = S.nlive[1] = 0;
 				}
 				const uint32_t w0 = (uint32_t)(bitpos >> 5);
-				stage_round(S.in, gwords, w0, nwords, nbytes);
+				stage_words(S.in, gwords, w0, kP1InWords, nwords, nbytes, tid, (int)blockDim.x);
 				__syncthreads();
 				const uint32_t *words = S.in;
 				const uint32_t r0 = (uint32_t)(bitpos & 31);
