@@ -324,6 +324,39 @@ int b200z_lzw_batch(const uint8_t *const *in, const int64_t *in_len, int32_t n, 
 int b200z_lzw_batch_multi(const int32_t *devices, int32_t n_devices, const uint8_t *const *in, const int64_t *in_len, int32_t n,
                           uint8_t *const *out, const int64_t *out_cap, int64_t *out_len, int64_t *in_used, uint32_t *value,
                           int32_t *status);
+/* ---------------------------------------------------------------------------------------------------------------
+ * Deflater sets -- n independent Deflater streams that arrive in pieces (a server compressing many responses or logs as
+ * they are written, a ZipOutputStream per client), run together: what N Deflater handles do, in one device pass per call.
+ * create: n streams of one level / strategy / wrap (RAW, ZLIB, GZIP, RAW_CRC32), each as fresh as new Deflater(level,
+ * raw); level -1 means 6.  The set is bound to the device b200z_init chose for the calling thread, like a pipeline;
+ * without a device B200Z_E_CUDA.
+ * write: per stream, SetInput(in[i], len[i]) drained as DeflaterOutputStream.Write does (Streams/DeflaterOutputStream.cs
+ * :245-275, so undrained_last is always 0), then op[i]: 0 = nothing more, 1 = Flush(), 2 = Finish().  len[i] may be 0.
+ * A stream with len[i] = 0 and op[i] = 0 is not written to, finished or not.  A finished stream takes nothing else:
+ * input or an op gives status[i] = B200Z_E_STATE, the other streams go on, and the call returns B200Z_E_STATE.  The
+ * streams with no Flush() / Finish() run an open run once they hold 4.25 MiB beyond the bytes their last run left behind
+ * its cut; the run takes at most that much more (levels 0-4: up to the end of the write it reaches into).  The open runs,
+ * then the flushes, then the finishes run as plans of at most 1 GiB of input each (a longer segment alone), one after the
+ * other on a CUDA stream of the set's own; each plan synchronises that stream twice.  A failed run leaves the set
+ * unusable: every later write returns its status.
+ * read: hands out what each stream has produced so far: out[i] gets min(cap[i], pending) bytes, got[i] the count.  For
+ * every stream the concatenation of everything read hands out is the reference's output for the same calls: with
+ * wrap = B200Z_WRAP_GZIP GZipOutputStream's (header with MTIME 0 and no FNAME, raw stream, CRC-32, ISIZE), otherwise
+ * Deflater's (zlib header and Adler-32 for ZLIB).  Output may come out later than the reference's, as with the handle.
+ * check: per stream the Adler-32 (ZLIB) or CRC-32 (GZIP, RAW_CRC32: a zip entry's crc) of the bytes compressed so far,
+ * of all of them once the stream has finished; 0 for RAW.
+ * stats: v[0] stream runs (segments compressed), v[1] plans run, v[2] the most input bytes one stream held at once,
+ * v[3] the most device workspace one plan took (bytes). 
+ * One set = one host thread at a time. */
+typedef struct b200z_deflate_streams b200z_deflate_streams;
+int b200z_deflate_streams_create(int32_t n, int level, int strategy, int wrap, b200z_deflate_streams **s);
+int b200z_deflate_streams_write(b200z_deflate_streams *s, const uint8_t *const *in, const int64_t *len, const int32_t *op,
+                                int32_t *status);
+int b200z_deflate_streams_read(b200z_deflate_streams *s, uint8_t *const *out, const int64_t *cap, int64_t *got);
+int b200z_deflate_streams_check(b200z_deflate_streams *s, uint32_t *check);
+int b200z_deflate_streams_stats(b200z_deflate_streams *s, int64_t *v, int32_t cap);
+int b200z_deflate_streams_destroy(b200z_deflate_streams *s);
+
 /* worst-case compressed size for `len` input bytes at any level (capacity a caller should provide) */
 int64_t b200z_deflate_bound(int64_t len);
 

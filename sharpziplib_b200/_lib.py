@@ -158,6 +158,12 @@ _SIGS = {
     "b200z_inflater_total_out": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "b200z_inflater_adler": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32)]),
     "b200z_inflater_get_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
+    "b200z_deflate_streams_create": (C.c_int, [C.c_int32, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "b200z_deflate_streams_write": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_deflate_streams_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_deflate_streams_check": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200z_deflate_streams_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
+    "b200z_deflate_streams_destroy": (C.c_int, [C.c_void_p]),
     "b200z_lzw_plan_create": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     "b200z_lzw_pipeline_create": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
     "b200z_lzw_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -277,6 +277,71 @@ def _ptr_array(arrs):
     return (C.c_void_p * len(arrs))(*[a.ctypes.data if a.size else None for a in arrs])
 
 
+class DeflaterSet:
+    """n independent Deflater streams of one level / strategy / wrap that arrive in pieces, run together on the device
+    (b200z_deflate_streams_*): what n Deflater objects behind DeflaterOutputStream (GZipOutputStream for WRAP_GZIP) do,
+    with one device pass per write() instead of one per stream."""
+    NOTHING, FLUSH, FINISH = 0, 1, 2
+
+    def __init__(self, n, level=6, strategy=0, wrap=_lib.WRAP_ZLIB):
+        h = C.c_void_p()
+        _lib.raise_for(_lib.lib().b200z_deflate_streams_create(n, level, strategy, wrap, C.byref(h)))
+        self._h = h
+        self.n = n
+        self.status = np.zeros(n, dtype=np.int32)  # per stream, of the last write()
+        self._cap = np.full(n, 65536, dtype=np.int64)
+
+    def write(self, buffers, ops=None):
+        """Write(buffers[i]) on every stream, then ops[i]: 0 nothing, 1 Flush(), 2 Finish() (None: all 0).  An empty
+        buffer with op 0 is no call, also for a finished stream.  A finished stream takes nothing else: its status is
+        E_STATE, the others go on, and InvalidOperationException is raised after."""
+        if len(buffers) != self.n or (ops is not None and len(ops) != self.n):
+            raise ValueError("one buffer and one op per stream")
+        ins = [np.ascontiguousarray(np.frombuffer(b, dtype=np.uint8)) for b in buffers]
+        lens = np.array([a.size for a in ins], dtype=np.int64)
+        op = np.zeros(self.n, dtype=np.int32) if ops is None else np.ascontiguousarray(ops, dtype=np.int32)
+        _lib.raise_for(_lib.lib().b200z_deflate_streams_write(self._h, _ptr_array(ins), lens.ctypes.data, op.ctypes.data,
+                                                               self.status.ctypes.data))
+
+    def read(self):
+        """everything each stream has produced since the last read(), as a list of bytes"""
+        parts = [[] for _ in range(self.n)]
+        want = np.ones(self.n, dtype=bool)
+        got = np.zeros(self.n, dtype=np.int64)
+        while want.any():
+            cap = np.where(want, self._cap, 0).astype(np.int64)
+            outs = [np.empty(int(c), dtype=np.uint8) for c in cap]
+            _lib.raise_for(_lib.lib().b200z_deflate_streams_read(self._h, _ptr_array(outs), cap.ctypes.data, got.ctypes.data))
+            for i in np.nonzero(want)[0]:
+                parts[i].append(outs[i][:got[i]].tobytes())
+            want &= got == cap
+            self._cap = np.where(want, np.minimum(self._cap * 4, 16 << 20), self._cap)
+        return [b"".join(p) for p in parts]
+
+    def checks(self):
+        """per stream: Adler-32 (WRAP_ZLIB) or CRC-32 (WRAP_GZIP, WRAP_RAW_CRC32) of the bytes compressed so far"""
+        v = np.zeros(self.n, dtype=np.uint32)
+        _lib.raise_for(_lib.lib().b200z_deflate_streams_check(self._h, v.ctypes.data))
+        return [int(x) for x in v]
+
+    def stats(self):
+        """{"runs": stream segments compressed, "plans": plans run, "held": most input bytes one stream held at once,
+        "workspace": most device workspace one plan took}"""
+        v = np.zeros(4, dtype=np.int64)
+        _lib.raise_for(_lib.lib().b200z_deflate_streams_stats(self._h, v.ctypes.data, 4))
+        return {"runs": int(v[0]), "plans": int(v[1]), "held": int(v[2]), "workspace": int(v[3])}
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                _lib.lib().b200z_deflate_streams_destroy(h)
+            except Exception:  # interpreter shutdown: the module globals may already be gone
+                pass
+
+    __del__ = close
+
+
 def deflate_batch(buffers, level=6, strategy=0, wrap=_lib.WRAP_RAW, end_mode=_lib.END_FINISH, devices=None):
     """Host buffers in, list of compressed bytes out (b200z_deflate_batch: H2D, kernels, D2H inside the call).
     devices: a list of CUDA device indices -- the batch is cut by bytes and every range runs on its own GPU at the same

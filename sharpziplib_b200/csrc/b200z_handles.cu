@@ -1,5 +1,6 @@
 // b200z_handles.cu -- the streaming handles of the C-ABI (include/b200z.h), which mirror Deflater.cs / Inflater.cs member
-// for member.  Each handle runs its plans synchronously from host buffers through one Staging (b200z_host.cuh).
+// for member, and the Deflater sets, which run many Deflater streams through the same host path.  Each handle runs its
+// plans synchronously from host buffers through one Staging (b200z_host.cuh), and so does a set.
 #include <algorithm>
 #include <cstring>
 
@@ -89,13 +90,308 @@ static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const ui
 }
 
 // =====================================================================================================
+// Deflater streams: the Deflater handle and the Deflater set share one host path
+// =====================================================================================================
+constexpr b200z_parse_entry kCleanEntry = {0, kMinMatch - 1, 0};
+
+// What one Deflater stream carries between device runs, whoever drives it (a handle, or a stream of a set).
+struct StreamCarry {
+	// what the engine's window has seen so far, cut to its last 32768 bytes (preset dictionary, then every compressed
+	// segment); hist_mask flags the positions InsertString never saw (the last two of the dictionary / of each segment)
+	std::vector<uint8_t> history, hist_mask;
+	int64_t window_seen = 0; // dictionary bytes kept + TotalIn: the SlideWindow phase of the next segment
+	bool started = false;    // an earlier segment (possibly empty) has been emitted
+	std::vector<uint8_t> input; // everything SetInput handed over and not yet compressed
+	// the parse state the next run starts from (levels 5-9), and the bytes at the front of `input` that the last open run
+	// saw but left behind its cut
+	b200z_parse_entry entry = kCleanEntry;
+	int64_t carried = 0;
+	// levels 0-4 depend on the call pattern (trap T9) and keep engine state across Flush() and cuts: the sizes of the SetInput
+	// calls in `input` (behind a cut the first is the rest of the call the cut fell into), whether Deflate() was called behind
+	// the last of them, and what the engines carry
+	std::vector<int64_t> chunks;
+	bool undrained = false;
+	b200z_stored_state sstate = {1, 1, 0, 0}; // level 0 (DeflateStored; a fresh engine: strstart = blockStart = 1)
+	DevBuf fstate;                            // levels 1-4 (DeflateFast: head[], prev[], scalars), on the device
+	std::vector<uint8_t> pending; // produced bytes not yet handed out
+	size_t pending_pos = 0;
+	HostBits tail;                // sub-byte tail carried between device runs
+	int64_t total_in = 0;
+	uint32_t check = 1;           // the running Adler-32 (zlib) or CRC-32 (gzip, raw + CRC-32)
+	void reset(uint32_t check0) { // (keeps the device buffer)
+		history.clear();
+		hist_mask.clear();
+		window_seen = 0;
+		started = false;
+		input.clear();
+		entry = kCleanEntry;
+		carried = 0;
+		chunks.clear();
+		undrained = false;
+		sstate = b200z_stored_state{1, 1, 0, 0};
+		pending.clear();
+		pending_pos = 0;
+		tail = HostBits();
+		total_in = 0;
+		check = check0;
+	}
+};
+
+static void carry_remember(StreamCarry *c, const uint8_t *seg, size_t len, size_t uninserted) {
+	// append a dictionary/segment to the carried window image
+	c->history.insert(c->history.end(), seg, seg + len);
+	c->hist_mask.insert(c->hist_mask.end(), len, 0);
+	for (size_t k = 0; k < uninserted && k < len; k++) c->hist_mask[c->hist_mask.size() - 1 - k] = 1;
+	if (c->history.size() > 32768) {
+		const size_t cut = c->history.size() - 32768;
+		c->history.erase(c->history.begin(), c->history.begin() + (ptrdiff_t)cut);
+		c->hist_mask.erase(c->hist_mask.begin(), c->hist_mask.begin() + (ptrdiff_t)cut);
+	}
+	c->window_seen += (int64_t)len;
+}
+
+// The bytes an open run may take: levels 0-4 whole SetInput calls whose Deflate() already ran (a call that Flush() /
+// Finish() follows directly stays with the closing run, b200z_history.undrained_last), levels 5-9 all of `input`.
+static int64_t open_run_avail(const StreamCarry *c, int level, int32_t *ncalls) {
+	*ncalls = (int32_t)c->chunks.size() - ((level <= 4 && c->undrained && !c->chunks.empty()) ? 1 : 0);
+	if (level >= 5) return (int64_t)c->input.size();
+	int64_t avail = 0;
+	for (int32_t k = 0; k < *ncalls; k++) avail += c->chunks[(size_t)k];
+	return avail;
+}
+
+// The length of an open run that takes the carried bytes plus at most `most` more of `avail` (> most).  It is longer than a
+// block can be, so it always ends in a cut and no run is repeated on the same bytes.  Levels 0-4 take enough whole calls to
+// close a block, however long the last one is; *ncalls becomes the number taken.
+static int64_t open_run_len(const StreamCarry *c, int level, int64_t avail, int64_t most, int32_t *ncalls) {
+	const int64_t len = std::min<int64_t>(avail, c->carried + most);
+	if (level >= 5) return len;
+	int64_t sum = 0;
+	int32_t k = 0;
+	// (more than one block's reach behind the carried bytes: the run closes a block)
+	const int64_t least = c->carried + (int64_t)kBlockSyms * kMaxMatch + kMaxMatch + kMinMatch + 1;
+	while (k < *ncalls && (sum < least || sum + c->chunks[(size_t)k] <= len)) sum += c->chunks[(size_t)k++];
+	*ncalls = k;
+	return sum;
+}
+
+// One device run of the next segment of k streams of one level / strategy / end mode, as one plan: segments_begin builds
+// the plan and enqueues the upload and the kernels on `cs`; segments_end waits for them, reads the cuts of an open run,
+// carries each stream's running checksum over the bytes its run covered and appends the produced bytes to its `pending`.
+// A run synchronises `cs` twice: once for the run's lengths and cuts, once for the produced bytes and checksums.
+// wrap is B200Z_WRAP_RAW, _ZLIB (the checksum is an Adler-32) or _RAW_CRC32 (a CRC-32).
+struct SegmentRun {
+	int level = 6, strategy = 0, wrap = B200Z_WRAP_RAW, end_mode = B200Z_END_FINISH;
+	std::vector<StreamCarry *> s;
+	std::vector<int64_t> len;   // per stream: the first len[i] bytes of its input (levels 0-4: its first calls[i] SetInput calls)
+	std::vector<int32_t> calls;
+	b200z_plan *plan = nullptr;
+	std::vector<b200z_stored_state> sbefore; // level 0: each state as the plan rebases it
+	SegmentRun() = default;
+	SegmentRun(const SegmentRun &) = delete;
+	~SegmentRun() { b200z_plan_destroy(plan); }
+	void add(StreamCarry *c, int64_t n, int32_t ncalls) {
+		s.push_back(c);
+		len.push_back(n);
+		calls.push_back(ncalls);
+	}
+};
+
+static int segments_begin(SegmentRun &r, Staging &st, cudaStream_t cs) {
+	const int k = (int)r.s.size();
+	const bool open = r.end_mode == B200Z_END_NONE;
+	bool any_started = false, any_hist = false;
+	for (const StreamCarry *c : r.s) {
+		any_started |= c->started;
+		any_hist |= !c->history.empty();
+	}
+	// A fresh stream next to continuing ones continues from nothing: no history, the fresh engine state
+	const int kind = any_started ? B200Z_HIST_CONTINUE : (any_hist ? B200Z_HIST_DICTIONARY : B200Z_HIST_NONE);
+	std::vector<int64_t> H((size_t)k), pos_base((size_t)k);
+	std::vector<int32_t> bit_base((size_t)k), undrained((size_t)k);
+	std::vector<const uint8_t *> mask((size_t)k), inp((size_t)k);
+	std::vector<const int64_t *> chunk_ptr((size_t)k);
+	std::vector<void *> fstate_ptr((size_t)k);
+	std::vector<b200z_stored_state> sstate((size_t)k);
+	std::vector<uint32_t> seed((size_t)k);
+	std::vector<b200z_parse_entry> entry((size_t)k);
+	std::vector<std::vector<uint8_t>> slot((size_t)k);
+	r.sbefore.resize((size_t)k);
+	for (int i = 0; i < k; i++) {
+		StreamCarry *c = r.s[(size_t)i];
+		if (kind == B200Z_HIST_CONTINUE && !c->started && !c->history.empty()) {
+			set_error("a stream with a preset dictionary cannot start in a run with continuing streams");
+			return B200Z_E_INTERNAL;
+		}
+		H[(size_t)i] = (int64_t)c->history.size();
+		pos_base[(size_t)i] = c->window_seen;
+		bit_base[(size_t)i] = c->tail.count;
+		mask[(size_t)i] = c->hist_mask.data();
+		chunk_ptr[(size_t)i] = c->chunks.data();
+		undrained[(size_t)i] = (c->undrained && r.calls[(size_t)i] == (int32_t)c->chunks.size() && r.calls[(size_t)i] > 0 && !open) ? 1 : 0;
+		if (r.level >= 1 && r.level <= 4) {
+			int rc = c->fstate.ensure((size_t)b200z_engine_state_bytes());
+			if (rc) return rc;
+			fstate_ptr[(size_t)i] = c->fstate.p;
+			if (kind == B200Z_HIST_CONTINUE && !c->started) { // DeflateFast as the constructor leaves it (fe_init)
+				const FastCarry fresh = {1, 1, 0, 0, kMinMatch - 1, 0, 0u, 0u};
+				B200Z_CUDA(cudaMemsetAsync(c->fstate.p, 0, 131072, cs));
+				B200Z_CUDA(cudaMemcpyAsync(c->fstate.p + 131072, &fresh, sizeof fresh, cudaMemcpyHostToDevice, cs));
+			}
+		}
+		sstate[(size_t)i] = c->sstate;
+		// level 0: the state as the plan rebases it, for the bytes a closing run takes (see stored_run)
+		r.sbefore[(size_t)i] = c->sstate;
+		if (c->started) carry_rebase(r.sbefore[(size_t)i].slides, r.sbefore[(size_t)i].input_off);
+		seed[(size_t)i] = c->check;
+		entry[(size_t)i] = c->entry;
+		inp[(size_t)i] = c->input.data();
+		if (H[(size_t)i]) {
+			std::vector<uint8_t> &v = slot[(size_t)i];
+			v.reserve((size_t)(H[(size_t)i] + r.len[(size_t)i]));
+			v.insert(v.end(), c->history.begin(), c->history.end());
+			v.insert(v.end(), c->input.begin(), c->input.begin() + r.len[(size_t)i]);
+			inp[(size_t)i] = v.data();
+		}
+	}
+	b200z_history hs;
+	memset(&hs, 0, sizeof hs);
+	if (r.level <= 4) {
+		hs.chunk_count = r.calls.data();
+		hs.chunk_len = chunk_ptr.data();
+		hs.undrained_last = undrained.data();
+		if (r.level == 0) hs.stored_state = sstate.data();
+		else hs.engine_state = fstate_ptr.data();
+	}
+	hs.kind = kind;
+	hs.check_seeded = 1;
+	hs.hist_len = H.data();
+	hs.pos_base = pos_base.data();
+	hs.bit_base = bit_base.data();
+	hs.hist_mask = mask.data();
+	int rc = b200z_deflate_plan_create_ex(k, r.len.data(), r.level, r.strategy, r.wrap, r.end_mode,
+	                                      (kind != B200Z_HIST_NONE || r.level <= 4) ? &hs : nullptr, &r.plan);
+	if (rc) return rc;
+	if (r.level == 0) // (the plan wrote the state behind this segment when it was created)
+		for (int i = 0; i < k; i++) r.s[(size_t)i]->sstate = sstate[(size_t)i];
+	if (r.level >= 5 && (rc = b200z_deflate_plan_set_entry(r.plan, entry.data()))) return rc;
+	// a plan with history continues the running checksum (hs.check_seeded)
+	if ((rc = st.ensure(r.plan, false))) return rc;
+	return stage_run(r.plan, st, inp.data(), false, (kind != B200Z_HIST_NONE && r.wrap != B200Z_WRAP_RAW && !open) ? seed.data() : nullptr,
+	                 cs, cs, nullptr);
+}
+
+static int segments_end(SegmentRun &r, Staging &st, cudaStream_t cs) {
+	const int k = (int)r.s.size();
+	const bool open = r.end_mode == B200Z_END_NONE;
+	B200Z_CUDA(cudaStreamSynchronize(cs));
+	const PipeMeta &m = st.h;
+	for (int i = 0; i < k; i++)
+		if ((m.status[i] & 0xFF) != B200Z_OK) {
+			set_error("device deflate failed with status %d", m.status[i] & 0xFF);
+			return m.status[i] & 0xFF;
+		}
+	std::vector<int64_t> covered(r.len); // bytes of input each run is done with
+	std::vector<b200z_parse_entry> next((size_t)k, kCleanEntry);
+	std::vector<int32_t> cut_call((size_t)k, 0);
+	std::vector<uint32_t> ck; // open runs: the running checksums behind the covered bytes
+	int rc = B200Z_OK;
+	if (open) {
+		rc = b200z_deflate_plan_get_cut(r.plan, covered.data(), r.level >= 5 ? next.data() : nullptr, cs);
+		if (!rc && r.level <= 4) rc = b200z_deflate_plan_get_cut_call(r.plan, cut_call.data(), cs);
+		if (rc) return rc;
+		for (int i = 0; i < k; i++)
+			if (covered[(size_t)i] <= 0) { // (a run of more than 16384 * 258 + 262 bytes always closes a block)
+				set_error("open run of %lld bytes closed no block", (long long)r.len[(size_t)i]);
+				return B200Z_E_INTERNAL;
+			}
+		if (r.wrap != B200Z_WRAP_RAW) {
+			// the checksums go on over the covered bytes, read from the copy of the input the run left on the device; the
+			// values come back with the produced bytes (streams_down synchronises once for both)
+			ck.resize((size_t)k);
+			std::vector<int64_t> off((size_t)k);
+			for (int i = 0; i < k; i++) {
+				ck[(size_t)i] = r.s[(size_t)i]->check;
+				off[(size_t)i] = b200z_plan_data_offset(r.plan, i);
+			}
+			B200Z_CUDA(cudaMemcpyAsync(st.d.check, ck.data(), 4ull * k, cudaMemcpyHostToDevice, cs));
+			if ((rc = b200z_checksum_batch_device(r.wrap == B200Z_WRAP_ZLIB ? 1 : 0, st.din.p, off.data(), covered.data(), k, st.d.check, cs)))
+				return rc;
+			B200Z_CUDA(cudaMemcpyAsync(ck.data(), st.d.check, 4ull * k, cudaMemcpyDeviceToHost, cs));
+		}
+	}
+	if ((rc = streams_down(r.plan, st, nullptr, cs))) return rc;
+	for (size_t i = 0; i < ck.size(); i++) r.s[i]->check = ck[i];
+	for (int i = 0; i < k; i++) {
+		StreamCarry *c = r.s[(size_t)i];
+		const int64_t len = r.len[(size_t)i], cov = covered[(size_t)i];
+		const uint8_t *o = st.hout.p + r.plan->out_off[(size_t)i];
+		const int64_t bits = m.in_used[i]; // deflate plans report the exact bit length here (bit_base included)
+		const int64_t whole = bits >> 3;
+		std::vector<uint8_t> seg(o, o + ((bits + 7) >> 3));
+		if (!seg.empty()) seg[0] |= (uint8_t)c->tail.bits; // the carried sub-byte tail completes the first byte
+		c->pending.insert(c->pending.end(), seg.begin(), seg.begin() + (ptrdiff_t)whole);
+		// PendingBuffer keeps the sub-byte tail in `bits` until later writes complete the byte (:168-189)
+		c->tail.count = (int)(bits & 7);
+		c->tail.bits = c->tail.count ? (seg[(size_t)whole] & ((1u << c->tail.count) - 1u)) : 0u;
+		if (r.end_mode == B200Z_END_FINISH) c->tail.align(c->pending); // FINISHING_STATE: AlignToByte (:507)
+		if (r.wrap != B200Z_WRAP_RAW && !open) c->check = m.check[i];
+		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run;
+		// the data starts strstart - block_start bytes in front of the state's input_off)
+		const b200z_stored_state &sb = r.sbefore[(size_t)i];
+		c->total_in += (r.level == 0 && !open) ? (int64_t)(uint32_t)(c->sstate.input_off - sb.input_off) + (sb.strstart - sb.block_start) : cov;
+		c->started = true;
+		// every position in front of a cut went through InsertString; a flush leaves the last two out
+		carry_remember(c, c->input.data(), (size_t)cov, open ? 0 : 2);
+		c->input.erase(c->input.begin(), c->input.begin() + cov);
+		c->entry = next[(size_t)i];
+		c->carried = len - cov;
+		if (!open) {
+			c->chunks.clear();
+			c->undrained = false;
+		} else if (r.level <= 4) {
+			// the next run's schedule: the rest of the call the cut fell into, then the calls behind it
+			int64_t end = 0;
+			for (int32_t j = 0; j <= cut_call[(size_t)i]; j++) end += c->chunks[(size_t)j];
+			c->chunks.erase(c->chunks.begin(), c->chunks.begin() + cut_call[(size_t)i]);
+			c->chunks[0] = end - cov;
+		}
+	}
+	return B200Z_OK;
+}
+
+// Finish() right behind a completed Flush(): every block and the sync padding are out, Finish adds the final empty block:
+// levels 1-9 FlushBlock on an empty buffer = static header 011 + EOB 0000000 = value 3 in 10 bits (DeflaterEngine.cs:750-768);
+// level 0 an empty stored block 01 00 00 FF FF (:614-649)
+static void final_empty_block(StreamCarry *c, int level) {
+	if (level == 0) {
+		const uint8_t e5[5] = {1, 0, 0, 0xFF, 0xFF};
+		c->pending.insert(c->pending.end(), e5, e5 + 5);
+	} else {
+		c->tail.put(c->pending, 3, 10);
+		c->tail.align(c->pending);
+	}
+}
+
+// behind the final block: zlib's Adler-32, big endian (Deflater.cs:509-514); gzip's CRC-32 and ISIZE = TotalIn & 0xFFFFFFFF,
+// little endian (GZipOutputStream.GetFooter, :315-337); nothing for a raw stream
+static void stream_trailer(StreamCarry *c, int wrap) {
+	if (wrap == B200Z_WRAP_ZLIB) {
+		for (int sh = 24; sh >= 0; sh -= 8) c->pending.push_back((uint8_t)(c->check >> sh));
+	} else if (wrap == B200Z_WRAP_GZIP) {
+		const uint32_t isz = (uint32_t)((uint64_t)c->total_in & 0xFFFFFFFFull);
+		for (int sh = 0; sh < 32; sh += 8) c->pending.push_back((uint8_t)(c->check >> sh));
+		for (int sh = 0; sh < 32; sh += 8) c->pending.push_back((uint8_t)(isz >> sh));
+	}
+}
+
+// =====================================================================================================
 // Streaming handles
 // =====================================================================================================
 // A long stream is compressed in open runs (B200Z_END_NONE) of this many new bytes, plus what the run in front left behind
 // its cut: a plan's workspace grows with its input (about 3.7 GB for 256 MiB at levels 5-9), the host holds no more than
 // that, and the output flows while input arrives.  A segment up to this size runs as one plan, as it always has.
 constexpr int64_t kOpenRunBytes = 256ll << 20;
-constexpr b200z_parse_entry kCleanEntry = {0, kMinMatch - 1, 0};
 
 struct DeflaterH {
 	int level = 6, strategy = 0;
@@ -104,206 +400,184 @@ struct DeflaterH {
 	bool flushing = false, finishing = false, finished = false;
 	bool header_done = false;
 	bool flushed_once = false; // a sync flush has been emitted and nothing was compressed since
-	// what the engine's window has seen so far, cut to its last 32768 bytes (preset dictionary, then every compressed
-	// segment); hist_mask flags the positions InsertString never saw (the last two of the dictionary / of each segment)
-	std::vector<uint8_t> history, hist_mask;
-	int64_t window_seen = 0;  // dictionary bytes kept + TotalIn: the SlideWindow phase of the next segment
-	bool dict_set = false, deflate_called = false, started = false;
+	bool dict_set = false, deflate_called = false;
 	uint32_t dict_adler = 0;
-	std::vector<uint8_t> input;    // everything SetInput handed over and not yet compressed
-	// the parse state the next run starts from (levels 5-9), the bytes at the front of `input` that the last open run saw
-	// but left behind its cut, and whether that run's output is still being handed out
-	b200z_parse_entry entry = kCleanEntry;
-	int64_t carried = 0;
-	bool draining = false;
-	std::vector<uint8_t> pending;  // produced bytes not yet drained by Deflate()
-	size_t pending_pos = 0;
-	HostBits tail;                 // sub-byte tail carried between device runs
-	int64_t total_in = 0, total_out = 0;
-	uint32_t adler = 1;
-	// levels 0-4 depend on the call pattern (trap T9) and keep engine state across Flush() and cuts: the sizes of the SetInput
-	// calls in `input` (behind a cut the first is the rest of the call the cut fell into), whether Deflate() was called behind
-	// the last of them, and what the engines carry
-	std::vector<int64_t> chunks;
-	bool undrained = false;
-	b200z_stored_state sstate = {0, 0, 0, 0}; // level 0 (DeflateStored)
-	DevBuf fstate;                            // levels 1-4 (DeflateFast: head[], prev[], scalars), on the device
+	bool draining = false; // the output of an open run is still being handed out
+	int64_t total_out = 0;
+	StreamCarry s;
 	Staging st;
 };
-
-static void deflater_remember(DeflaterH *d, const uint8_t *seg, size_t len, size_t uninserted) {
-	// append a dictionary/segment to the carried window image
-	d->history.insert(d->history.end(), seg, seg + len);
-	d->hist_mask.insert(d->hist_mask.end(), len, 0);
-	for (size_t k = 0; k < uninserted && k < len; k++) d->hist_mask[d->hist_mask.size() - 1 - k] = 1;
-	if (d->history.size() > 32768) {
-		const size_t cut = d->history.size() - 32768;
-		d->history.erase(d->history.begin(), d->history.begin() + (ptrdiff_t)cut);
-		d->hist_mask.erase(d->hist_mask.begin(), d->hist_mask.begin() + (ptrdiff_t)cut);
-	}
-	d->window_seen += (int64_t)len;
-}
 
 static void deflater_header(DeflaterH *d) {
 	if (!d->header_done && !d->raw) {
 		uint8_t hd[2];
 		zlib_header(d->level, hd, d->dict_set);
-		d->pending.push_back(hd[0]);
-		d->pending.push_back(hd[1]);
+		d->s.pending.push_back(hd[0]);
+		d->s.pending.push_back(hd[1]);
 		if (d->dict_set) { // DICTID = Adler-32 of the whole dictionary, MSB first (:455-461)
-			for (int sh = 24; sh >= 0; sh -= 8) d->pending.push_back((uint8_t)(d->dict_adler >> sh));
+			for (int sh = 24; sh >= 0; sh -= 8) d->s.pending.push_back((uint8_t)(d->dict_adler >> sh));
 		}
 	}
 	d->header_done = true;
 }
 
+// compresses the first `len` bytes of the input (levels 0-4: the first n_chunks SetInput calls) as the next segment of the
+// stream, in a plan of its own on the legacy default stream; END_FLUSH keeps the stream open and may end inside a byte;
+// END_NONE writes the blocks that closed and keeps the bytes behind them for the next run
 static int deflater_run_device(DeflaterH *d, int end_mode, int64_t len, int32_t n_chunks) {
-	// compresses the first `len` bytes of d->input (levels 0-4: the first n_chunks SetInput calls) as the next segment of the
-	// stream; END_FLUSH keeps the stream open and may end inside a byte; END_NONE writes the blocks that closed and keeps the
-	// bytes behind them for the next run
-	const bool open = end_mode == B200Z_END_NONE;
-	const int64_t H = (int64_t)d->history.size();
-	const bool continuing = d->started; // an earlier segment (possibly empty) has been emitted
-	b200z_history hs;
-	memset(&hs, 0, sizeof hs);
-	const int64_t *chunk_ptr = d->chunks.data();
-	const int32_t undrained = (d->undrained && n_chunks == (int32_t)d->chunks.size() && n_chunks > 0 && !open) ? 1 : 0;
-	void *fstate_ptr = nullptr;
-	if (d->level <= 4) {
-		hs.chunk_count = &n_chunks;
-		hs.chunk_len = &chunk_ptr;
-		hs.undrained_last = &undrained;
-		if (d->level == 0) hs.stored_state = &d->sstate;
-		else {
-			int rc0 = d->fstate.ensure((size_t)b200z_engine_state_bytes());
-			if (rc0) return rc0;
-			fstate_ptr = d->fstate.p;
-			hs.engine_state = &fstate_ptr;
-		}
-	}
-	const int64_t pos_base = d->window_seen;
-	const int32_t bit_base = d->tail.count;
-	const uint8_t *mask = d->hist_mask.data();
-	hs.kind = continuing ? B200Z_HIST_CONTINUE : (H ? B200Z_HIST_DICTIONARY : B200Z_HIST_NONE);
-	hs.check_seeded = 1;
-	hs.hist_len = &H;
-	hs.pos_base = &pos_base;
-	hs.bit_base = &bit_base;
-	hs.hist_mask = &mask;
-	// level 0: the state as the plan rebases it, for the bytes a closing run takes (see stored_run)
-	b200z_stored_state sbefore = d->sstate;
-	if (continuing) carry_rebase(sbefore.slides, sbefore.input_off);
-	b200z_plan *plan = nullptr;
-	int rc = b200z_deflate_plan_create_ex(1, &len, d->level, d->strategy, d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB, end_mode,
-	                                      (hs.kind != B200Z_HIST_NONE || d->level <= 4) ? &hs : nullptr, &plan);
-	if (rc) return rc;
-	if (d->level >= 5) rc = b200z_deflate_plan_set_entry(plan, &d->entry);
-	std::vector<uint8_t> slot;
-	const uint8_t *inp = d->input.data();
-	if (H) {
-		slot.reserve((size_t)(H + len));
-		slot.insert(slot.end(), d->history.begin(), d->history.end());
-		slot.insert(slot.end(), d->input.begin(), d->input.begin() + len);
-		inp = slot.data();
-	}
-	const uint32_t seed = d->adler; // a plan with history continues the running checksum (hs.check_seeded)
-	if (!rc) rc = handle_run(plan, d->st, inp, (hs.kind != B200Z_HIST_NONE && !d->raw && !open) ? &seed : nullptr);
-	const PipeMeta &r = d->st.h;
-	if (!rc && (r.status[0] & 0xFF) != B200Z_OK) {
-		rc = r.status[0] & 0xFF;
-		set_error("device deflate failed with status %d", rc);
-	}
-	int64_t covered = len; // bytes of input this run is done with
-	b200z_parse_entry next = kCleanEntry;
-	int32_t cut_call = 0;
-	if (!rc && open) {
-		rc = b200z_deflate_plan_get_cut(plan, &covered, d->level >= 5 ? &next : nullptr, nullptr);
-		if (!rc && d->level <= 4) rc = b200z_deflate_plan_get_cut_call(plan, &cut_call, nullptr);
-		if (!rc && covered <= 0) { // (a run of more than 16384 * 258 + 262 bytes always closes a block)
-			set_error("open run of %lld bytes closed no block", (long long)len);
-			rc = B200Z_E_INTERNAL;
-		}
-		if (!rc && !d->raw) {
-			// the Adler-32 goes on over the covered bytes, read from the copy of the input the run left on the device
-			const int64_t off = b200z_plan_data_offset(plan, 0);
-			cudaError_t e = cudaMemcpy(d->st.d.check, &d->adler, 4, cudaMemcpyHostToDevice);
-			if (e == cudaSuccess && !(rc = b200z_checksum_batch_device(1, d->st.din.p, &off, &covered, 1, d->st.d.check, nullptr)))
-				e = cudaMemcpy(&d->adler, d->st.d.check, 4, cudaMemcpyDeviceToHost);
-			if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpy (running Adler-32)", __FILE__, __LINE__);
-		}
-	}
-	if (!rc) {
-		const uint8_t *o = d->st.hout.p + plan->out_off[0];
-		const int64_t bits = r.in_used[0]; // deflate plans report the exact bit length here (bit_base included)
-		const int64_t whole = bits >> 3;
-		std::vector<uint8_t> seg(o, o + ((bits + 7) >> 3));
-		if (!seg.empty()) seg[0] |= (uint8_t)d->tail.bits; // the carried sub-byte tail completes the first byte
-		d->pending.insert(d->pending.end(), seg.begin(), seg.begin() + (ptrdiff_t)whole);
-		// PendingBuffer keeps the sub-byte tail in `bits` until later writes complete the byte (:168-189)
-		d->tail.count = (int)(bits & 7);
-		d->tail.bits = d->tail.count ? (seg[(size_t)whole] & ((1u << d->tail.count) - 1u)) : 0u;
-		if (end_mode == B200Z_END_FINISH) d->tail.align(d->pending); // FINISHING_STATE: AlignToByte (:507)
-		if (!d->raw && !open) d->adler = r.check[0];
-		// (level 0: Finish() behind an undrained SetInput can end the stream before all input is taken, see stored_run;
-		// the data starts strstart - block_start bytes in front of the state's input_off)
-		d->total_in += (d->level == 0 && !open)
-		                   ? (int64_t)(uint32_t)(d->sstate.input_off - sbefore.input_off) + (sbefore.strstart - sbefore.block_start)
-		                   : covered;
-		d->started = true;
-		// every position in front of a cut went through InsertString; a flush leaves the last two out
-		deflater_remember(d, d->input.data(), (size_t)covered, open ? 0 : 2);
-		d->input.erase(d->input.begin(), d->input.begin() + covered);
-		d->entry = next;
-		d->carried = len - covered;
-		if (!open) {
-			d->chunks.clear();
-			d->undrained = false;
-		} else if (d->level <= 4) {
-			// the next run's schedule: the rest of the call the cut fell into, then the calls behind it
-			int64_t end = 0;
-			for (int32_t k = 0; k <= cut_call; k++) end += d->chunks[(size_t)k];
-			d->chunks.erase(d->chunks.begin(), d->chunks.begin() + cut_call);
-			d->chunks[0] = end - covered;
-		}
-	}
-	b200z_plan_destroy(plan);
-	return rc;
+	SegmentRun r;
+	r.level = d->level;
+	r.strategy = d->strategy;
+	r.wrap = d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB;
+	r.end_mode = end_mode;
+	r.add(&d->s, len, n_chunks);
+	int rc = segments_begin(r, d->st, 0);
+	return rc ? rc : segments_end(r, d->st, 0);
 }
 
 // While more than one run's worth of input is buffered, the front of it is compressed in open runs and their output is due
-// at once.  Each run takes the bytes its predecessor left behind the cut plus at most kOpenRunBytes more, so it is longer
-// than a block can be and always ends in a cut: no run is repeated on the same bytes.  Levels 0-4 take whole SetInput
-// calls whose Deflate() already ran (enough of them to close a block, however long the last one is): a call that Flush() /
-// Finish() follows directly stays with the closing run (b200z_history.undrained_last).
+// at once.  Each run takes the bytes its predecessor left behind the cut plus at most kOpenRunBytes more.
 static int deflater_open_runs(DeflaterH *d) {
 	for (;;) {
-		const bool fast = d->level <= 4;
-		int32_t ncalls = (int32_t)d->chunks.size() - ((fast && d->undrained && !d->chunks.empty()) ? 1 : 0);
-		int64_t avail = (int64_t)d->input.size();
-		if (fast) {
-			avail = 0;
-			for (int32_t k = 0; k < ncalls; k++) avail += d->chunks[(size_t)k];
-		}
+		int32_t ncalls = 0;
+		const int64_t avail = open_run_avail(&d->s, d->level, &ncalls);
 		if (avail <= kOpenRunBytes) return B200Z_OK;
-		int64_t len = std::min<int64_t>(avail, d->carried + kOpenRunBytes);
-		if (fast) {
-			int64_t sum = 0;
-			int32_t k = 0;
-			// (more than one block's reach behind the carried bytes: the run closes a block)
-			const int64_t least = d->carried + (int64_t)kBlockSyms * kMaxMatch + kMaxMatch + kMinMatch + 1;
-			while (k < ncalls && (sum < least || sum + d->chunks[(size_t)k] <= len)) sum += d->chunks[(size_t)k++];
-			len = sum;
-			ncalls = k;
-		}
-		if (d->pending_pos == d->pending.size()) {
-			d->pending.clear();
-			d->pending_pos = 0;
+		const int64_t len = open_run_len(&d->s, d->level, avail, kOpenRunBytes, &ncalls);
+		if (d->s.pending_pos == d->s.pending.size()) {
+			d->s.pending.clear();
+			d->s.pending_pos = 0;
 		}
 		deflater_header(d);
 		int rc = deflater_run_device(d, B200Z_END_NONE, len, ncalls);
 		if (rc) return rc;
 		d->draining = true;
 	}
+}
+
+// ---- Deflater set ------------------------------------------------------------------------------------
+// n Deflater streams of one level / strategy / wrap, driven together.  A write appends every stream's input as
+// DeflaterOutputStream.Write hands it over (SetInput, then Deflate() until it needs input); then the streams with enough
+// buffered run their open runs, the streams that flush their flushes and those that finish their finishes, each group in
+// as few plans as kSetPlanBytes allows, one after the other on the set's CUDA stream.  A stream with no Flush() / Finish()
+// due runs an open run once it holds kSetRunBytes beyond what it carries, and the run takes at most kSetRunBytes more than
+// that (levels 0-4 end a run at a SetInput call, so it may take the rest of the call it reaches into).  kSetRunBytes is more
+// than the 16384 * 258 + 262 bytes after which a run at levels 0-4 always closes a block.
+// A plan's device workspace grows with its input (at levels 5-9 about 14 bytes per input byte), so the streams of one
+// group are split into plans of at most kSetPlanBytes of input (history included; a stream longer than that runs alone):
+// 256 streams due at once, about 256 x 8.5 MiB at most, take two or three plans, whatever the number of streams.
+// (The CPU test tier builds the kernels on the CUDA emulator with smaller values, for small data.)
+#ifndef B200Z_SET_RUN_BYTES
+#define B200Z_SET_RUN_BYTES 4456448 // 4.25 MiB
+#endif
+#ifndef B200Z_SET_PLAN_BYTES
+#define B200Z_SET_PLAN_BYTES (1ll << 30)
+#endif
+constexpr int64_t kSetRunBytes = B200Z_SET_RUN_BYTES;
+constexpr int64_t kSetPlanBytes = B200Z_SET_PLAN_BYTES;
+
+struct SetStream : StreamCarry {
+	bool header_done = false, flushed_once = false, finished = false;
+};
+
+} // namespace b200z
+
+struct b200z_deflate_streams {
+	int device = -1, level = 6, strategy = 0, wrap = B200Z_WRAP_ZLIB;
+	std::vector<b200z::SetStream> s;
+	b200z::Staging st; // grows to the largest plan, at most kSetPlanBytes of input and its output bound, until destroy
+	cudaStream_t cs = nullptr;
+	int broken = 0; // a run failed: the streams' state is not what their output says, no more writes
+	int64_t stats[4] = {0, 0, 0, 0}; // b200z_deflate_streams_stats
+};
+
+namespace b200z {
+
+static void set_header(const b200z_deflate_streams *S, SetStream *c) {
+	if (c->header_done) return;
+	if (S->wrap == B200Z_WRAP_ZLIB) {
+		uint8_t hd[2];
+		zlib_header(S->level, hd);
+		c->pending.insert(c->pending.end(), hd, hd + 2);
+	} else if (S->wrap == B200Z_WRAP_GZIP) {
+		// GZipOutputStream's header (GzipOutputStream.cs:339-375) with MTIME 0 and no FNAME, as the pipelines write it
+		const uint8_t h[10] = {0x1F, 0x8B, 8, 0, 0, 0, 0, 0, 0, 0xFF};
+		c->pending.insert(c->pending.end(), h, h + 10);
+	}
+	c->header_done = true;
+}
+
+struct SetDue { // a stream's next segment: its first len bytes, in its first `calls` SetInput calls
+	SetStream *c;
+	int64_t len;
+	int32_t calls;
+};
+
+// runs the segments of one end mode in plans of at most kSetPlanBytes of input each
+static int set_plans(b200z_deflate_streams *S, int end_mode, const std::vector<SetDue> &due) {
+	for (size_t a = 0; a < due.size();) {
+		SegmentRun r;
+		r.level = S->level;
+		r.strategy = S->strategy;
+		r.wrap = S->wrap == B200Z_WRAP_GZIP ? B200Z_WRAP_RAW_CRC32 : S->wrap; // (gzip: the set writes header and trailer)
+		r.end_mode = end_mode;
+		int64_t bytes = 0;
+		for (; a < due.size(); a++) {
+			const int64_t b = due[a].len + (int64_t)due[a].c->history.size();
+			if (!r.s.empty() && bytes + b > kSetPlanBytes) break;
+			bytes += b;
+			set_header(S, due[a].c);
+			r.add(due[a].c, due[a].len, due[a].calls);
+		}
+		int rc = segments_begin(r, S->st, S->cs);
+		if (r.plan) S->stats[3] = std::max(S->stats[3], b200z_plan_workspace_bytes(r.plan));
+		if (!rc) rc = segments_end(r, S->st, S->cs);
+		if (rc) return rc;
+		S->stats[0] += (int64_t)r.s.size();
+		S->stats[1]++;
+	}
+	return B200Z_OK;
+}
+
+// the runs a write makes due; written[i] == 0 leaves stream i out
+static int set_runs(b200z_deflate_streams *S, const int32_t *op, const std::vector<char> &written) {
+	const int n = (int)S->s.size();
+	int rc;
+	for (;;) { // (a write of more than kSetRunBytes can need more than one open run)
+		std::vector<SetDue> due;
+		for (int i = 0; i < n; i++) {
+			SetStream *c = &S->s[(size_t)i];
+			int32_t ncalls = 0;
+			const int64_t avail = open_run_avail(c, S->level, &ncalls);
+			if (!written[(size_t)i] || avail - c->carried < kSetRunBytes) continue;
+			const int64_t len = open_run_len(c, S->level, avail, kSetRunBytes, &ncalls);
+			due.push_back(SetDue{c, len, ncalls});
+		}
+		if (due.empty()) break;
+		if ((rc = set_plans(S, B200Z_END_NONE, due))) return rc;
+	}
+	std::vector<SetDue> fl, fi;
+	for (int i = 0; i < n; i++) {
+		SetStream *c = &S->s[(size_t)i];
+		if (!written[(size_t)i] || op[i] == 0) continue;
+		const SetDue d{c, (int64_t)c->input.size(), (int32_t)c->chunks.size()};
+		if (op[i] == 1) fl.push_back(d);
+		else if (!c->flushed_once) fi.push_back(d);
+		else { // Finish() right behind a Flush(): no run
+			set_header(S, c);
+			final_empty_block(c, S->level);
+		}
+	}
+	if ((rc = set_plans(S, B200Z_END_FLUSH, fl)) || (rc = set_plans(S, B200Z_END_FINISH, fi))) return rc;
+	for (int i = 0; i < n; i++) {
+		SetStream *c = &S->s[(size_t)i];
+		if (!written[(size_t)i] || op[i] == 0) continue;
+		c->flushed_once = op[i] == 1;
+		if (op[i] == 2) {
+			stream_trailer(c, S->wrap);
+			c->finished = true;
+		}
+	}
+	return B200Z_OK;
 }
 
 // ---- Inflater handle ----------------------------------------------------------------------------------
@@ -504,23 +778,11 @@ int b200z_deflater_reset(void *h) { // Deflater.Reset :204-210 keeps level and s
 	d->flushing = d->finishing = d->finished = false;
 	d->header_done = false;
 	d->flushed_once = false;
-	d->input.clear();
-	d->pending.clear();
-	d->pending_pos = 0;
-	d->tail = HostBits();
-	d->total_in = d->total_out = 0;
-	d->adler = 1;
-	d->history.clear();
-	d->hist_mask.clear();
-	d->window_seen = 0;
-	d->dict_set = d->deflate_called = d->started = false;
+	d->total_out = 0;
+	d->dict_set = d->deflate_called = false;
 	d->dict_adler = 0;
-	d->chunks.clear();
-	d->undrained = false;
-	d->sstate = b200z_stored_state{0, 0, 0, 0};
-	d->entry = kCleanEntry;
-	d->carried = 0;
 	d->draining = false;
+	d->s.reset(1);
 	return B200Z_OK;
 }
 int b200z_deflater_set_level(void *h, int level) {
@@ -530,7 +792,7 @@ int b200z_deflater_set_level(void *h, int level) {
 		set_error("level");
 		return B200Z_E_ARG;
 	}
-	if (level != d->level && (!d->input.empty() || d->total_in > 0)) {
+	if (level != d->level && (!d->s.input.empty() || d->s.total_in > 0)) {
 		set_error("SetLevel in mid-stream (DeflaterEngine.SetLevel flushes a block, trap T17) is not accelerated");
 		return B200Z_E_UNSUPPORTED;
 	}
@@ -547,7 +809,7 @@ int b200z_deflater_set_strategy(void *h, int strategy) {
 		return B200Z_E_ARG;
 	}
 	DeflaterH *d = (DeflaterH *)h;
-	if (strategy != d->strategy && !d->input.empty()) {
+	if (strategy != d->strategy && !d->s.input.empty()) {
 		// the reference switches at the engine's current strstart (DeflaterEngine.cs:283-298), somewhere inside the input it
 		// holds -- like SetLevel in mid-stream; behind a completed Flush() the switch is exact and allowed
 		set_error("SetStrategy between SetInput and Flush()/Finish() is not accelerated");
@@ -560,7 +822,7 @@ int b200z_deflater_set_dictionary(void *h, const uint8_t *dict, int32_t len) {
 	DeflaterH *d = (DeflaterH *)h;
 	// Deflater.SetDictionary :372-381: only in INIT_STATE (before the header went out); the header's FDICT bit and
 	// DICTID come from the engine's Adler-32 over the dictionary, which is then reset (:386-401)
-	if (d->raw || d->deflate_called || d->header_done || d->total_in > 0 || d->dict_set) {
+	if (d->raw || d->deflate_called || d->header_done || d->s.total_in > 0 || d->dict_set) {
 		// state != INIT_STATE (:561): a raw deflater starts in BUSY_STATE (:206), Deflate() leaves INIT_STATE (:436-464)
 		set_error("SetDictionary: not in the initial state"); // InvalidOperationException
 		return B200Z_E_STATE;
@@ -578,7 +840,7 @@ int b200z_deflater_set_dictionary(void *h, const uint8_t *dict, int32_t len) {
 	d->dict_set = true;
 	if (len < kMinMatch) return B200Z_OK; // DeflaterEngine.cs:207-210: too short to matter, not even copied
 	const int32_t keep = len > kMaxDist ? kMaxDist : len; // :212-216
-	deflater_remember(d, dict + (len - keep), (size_t)keep, 2);
+	carry_remember(&d->s, dict + (len - keep), (size_t)keep, 2);
 	return B200Z_OK;
 }
 int b200z_deflater_set_input(void *h, const uint8_t *buf, int32_t len) {
@@ -594,12 +856,12 @@ int b200z_deflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 	// (no length limit: Deflate() runs long input in open runs, so a closing run holds at most what the last one carried,
 	// kOpenRunBytes and one SetInput of at most 2^31 - 1 bytes, and plans take a stream position of any size)
 	if (len > 0) d->flushed_once = false;
-	d->input.insert(d->input.end(), buf, buf + len);
+	d->s.input.insert(d->s.input.end(), buf, buf + len);
 	if (len > 0) {
 		// engine.NeedsInput (DeflaterEngine.cs:187-190) is false until Deflate() has taken the bytes; a zero-length SetInput
 		// leaves it true, so the stream classes do not even call Deflate() for it
-		d->undrained = true;
-		if (d->level <= 4) d->chunks.push_back(len); // the schedule matters for DeflateStored / DeflateFast only (trap T9)
+		d->s.undrained = true;
+		if (d->level <= 4) d->s.chunks.push_back(len); // the schedule matters for DeflateStored / DeflateFast only (trap T9)
 	}
 	return B200Z_OK;
 }
@@ -621,54 +883,40 @@ int b200z_deflater_deflate(void *h, uint8_t *out, int32_t cap, int32_t *produced
 	}
 	*produced = 0;
 	d->deflate_called = true;
-	if (!d->flushing && !d->finishing) d->undrained = false; // BUSY_STATE: the engine takes everything SetInput handed over
+	if (!d->flushing && !d->finishing) d->s.undrained = false; // BUSY_STATE: the engine takes everything SetInput handed over
 	if (!d->finished) { // (also in front of a Flush() / Finish() run: no run sees more than one run's worth of new input)
 		int rc = deflater_open_runs(d);
 		if (rc) return rc;
 	}
 	// make output due (Deflater.Deflate :427-522)
-	if (!d->finished && d->pending_pos == d->pending.size() && (d->flushing || d->finishing)) {
-		d->pending.clear();
-		d->pending_pos = 0;
+	if (!d->finished && d->s.pending_pos == d->s.pending.size() && (d->flushing || d->finishing)) {
+		d->s.pending.clear();
+		d->s.pending_pos = 0;
 		deflater_header(d);
 		if (d->finishing) {
 			if (d->flushed_once) {
-				// Flush() already emitted every block + the sync padding; Finish adds the final empty block:
-				// levels 1-9 FlushBlock on an empty buffer = static header 011 + EOB 0000000 = value 3 in 10 bits
-				// (DeflaterEngine.cs:750-768); level 0 an empty stored block 01 00 00 FF FF (:614-649)
-				if (d->level == 0) {
-					const uint8_t e5[5] = {1, 0, 0, 0xFF, 0xFF};
-					d->pending.insert(d->pending.end(), e5, e5 + 5);
-				} else {
-					d->tail.put(d->pending, 3, 10);
-					d->tail.align(d->pending);
-				}
+				final_empty_block(&d->s, d->level);
 			} else {
-				int rc = deflater_run_device(d, B200Z_END_FINISH, (int64_t)d->input.size(), (int32_t)d->chunks.size());
+				int rc = deflater_run_device(d, B200Z_END_FINISH, (int64_t)d->s.input.size(), (int32_t)d->s.chunks.size());
 				if (rc) return rc;
 			}
-			if (!d->raw) {
-				d->pending.push_back((uint8_t)(d->adler >> 24));
-				d->pending.push_back((uint8_t)(d->adler >> 16));
-				d->pending.push_back((uint8_t)(d->adler >> 8));
-				d->pending.push_back((uint8_t)d->adler);
-			}
+			stream_trailer(&d->s, d->raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB);
 			d->finished = true;
 		} else {
 			// sync flush (level 0 skips the padding, :488)
-			int rc = deflater_run_device(d, B200Z_END_FLUSH, (int64_t)d->input.size(), (int32_t)d->chunks.size());
+			int rc = deflater_run_device(d, B200Z_END_FLUSH, (int64_t)d->s.input.size(), (int32_t)d->s.chunks.size());
 			if (rc) return rc;
 			d->flushed_once = true;
 			d->flushing = false;
 		}
 	}
-	size_t avail = d->pending.size() - d->pending_pos;
+	size_t avail = d->s.pending.size() - d->s.pending_pos;
 	size_t take = avail < (size_t)cap ? avail : (size_t)cap;
-	if (take) memcpy(out, d->pending.data() + d->pending_pos, take);
-	d->pending_pos += take;
+	if (take) memcpy(out, d->s.pending.data() + d->s.pending_pos, take);
+	d->s.pending_pos += take;
 	d->total_out += (int64_t)take;
 	*produced = (int32_t)take;
-	if (d->pending_pos == d->pending.size()) d->draining = false;
+	if (d->s.pending_pos == d->s.pending.size()) d->draining = false;
 	return B200Z_OK;
 }
 int b200z_deflater_needs_input(void *h, int *flag) {
@@ -678,17 +926,17 @@ int b200z_deflater_needs_input(void *h, int *flag) {
 	// Flush() / Finish() changes the bytes at levels 0-4 (b200z_history.undrained_last).  The output of an open run also
 	// keeps it false until it has been handed out, as the reference's engine holds input while its output is pending.
 	const DeflaterH *d = (const DeflaterH *)h;
-	*flag = (d->undrained || d->draining) ? 0 : 1;
+	*flag = (d->s.undrained || d->draining) ? 0 : 1;
 	return B200Z_OK;
 }
 int b200z_deflater_is_finished(void *h, int *flag) {
 	DeflaterH *d = (DeflaterH *)h;
-	*flag = (d->finished && d->pending_pos == d->pending.size()) ? 1 : 0; // Deflater.cs:271-277
+	*flag = (d->finished && d->s.pending_pos == d->s.pending.size()) ? 1 : 0; // Deflater.cs:271-277
 	return B200Z_OK;
 }
 int b200z_deflater_total_in(void *h, int64_t *v) {
 	DeflaterH *d = (DeflaterH *)h;
-	*v = d->total_in;
+	*v = d->s.total_in;
 	return B200Z_OK;
 }
 int b200z_deflater_total_out(void *h, int64_t *v) {
@@ -697,7 +945,7 @@ int b200z_deflater_total_out(void *h, int64_t *v) {
 }
 int b200z_deflater_adler(void *h, uint32_t *v) {
 	DeflaterH *d = (DeflaterH *)h;
-	*v = d->raw ? 0u : d->adler;
+	*v = d->raw ? 0u : d->s.check;
 	return B200Z_OK;
 }
 
@@ -917,6 +1165,137 @@ int b200z_inflater_get_stats(void *h, int64_t *v, int32_t cap) {
 	}
 	const InflaterH *d = (const InflaterH *)h;
 	for (int32_t i = 0; i < cap && i < 4; i++) v[i] = d->stats[i];
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_create(int32_t n, int level, int strategy, int wrap, b200z_deflate_streams **s) {
+	if (!s || n < 0) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	if (level == -1) level = 6;
+	if (level < 0 || level > 9 || strategy < 0 || strategy > 2 || wrap < B200Z_WRAP_RAW || wrap > B200Z_WRAP_RAW_CRC32) {
+		set_error("level/strategy/wrap");
+		return B200Z_E_ARG;
+	}
+	int rc = ensure_init();
+	if (rc) return rc;
+	b200z_deflate_streams *S = new b200z_deflate_streams();
+	S->device = current_device();
+	DeviceGuard guard(S->device);
+	S->level = level;
+	S->strategy = strategy;
+	S->wrap = wrap;
+	S->s = std::vector<SetStream>((size_t)n);
+	for (SetStream &c : S->s) c.check = wrap == B200Z_WRAP_ZLIB ? 1u : 0u; // Adler32.Reset / Crc32.Reset
+	if (cudaStreamCreateWithFlags(&S->cs, cudaStreamNonBlocking) != cudaSuccess) {
+		delete S;
+		set_error("cudaStreamCreate failed");
+		return B200Z_E_CUDA;
+	}
+	*s = S;
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_write(b200z_deflate_streams *S, const uint8_t *const *in, const int64_t *len, const int32_t *op, int32_t *status) {
+	if (!S || (!S->s.empty() && (!in || !len || !op || !status))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	const int n = (int)S->s.size();
+	for (int i = 0; i < n; i++) // (nothing is taken when an argument is bad)
+		if (len[i] < 0 || (len[i] > 0 && !in[i]) || op[i] < 0 || op[i] > 2) {
+			set_error("stream %d: buffer/count/op", i);
+			return B200Z_E_ARG;
+		}
+	if (S->broken) {
+		set_error("an earlier run of this Deflater set failed with status %d", S->broken);
+		return S->broken;
+	}
+	DeviceGuard guard(S->device);
+	int first = -1;
+	std::vector<char> written((size_t)n, 0);
+	for (int i = 0; i < n; i++) {
+		SetStream &c = S->s[(size_t)i];
+		status[i] = B200Z_OK;
+		if (c.finished) { // Deflater.SetInput: "Finish() already called" (Deflater.cs:335); nothing at all is no call
+			if (len[i] > 0 || op[i] != 0) {
+				status[i] = B200Z_E_STATE;
+				if (first < 0) first = i;
+			}
+			continue;
+		}
+		written[(size_t)i] = 1;
+		c.input.insert(c.input.end(), in[i], in[i] + len[i]);
+		if (len[i] > 0) {
+			c.flushed_once = false;
+			if (S->level <= 4) c.chunks.push_back(len[i]); // the schedule (trap T9); every write drains, so none is undrained
+		}
+		S->stats[2] = std::max(S->stats[2], (int64_t)c.input.size());
+	}
+	const int rc = set_runs(S, op, written);
+	if (rc) {
+		S->broken = rc;
+		return rc;
+	}
+	if (first >= 0) {
+		set_error("stream %d: Finish() already called", first);
+		return B200Z_E_STATE;
+	}
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_read(b200z_deflate_streams *S, uint8_t *const *out, const int64_t *cap, int64_t *got) {
+	if (!S || (!S->s.empty() && (!out || !cap || !got))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	const int n = (int)S->s.size();
+	for (int i = 0; i < n; i++)
+		if (cap[i] < 0 || (cap[i] > 0 && !out[i])) {
+			set_error("stream %d: buffer/count", i);
+			return B200Z_E_ARG;
+		}
+	for (int i = 0; i < n; i++) {
+		SetStream &c = S->s[(size_t)i];
+		const int64_t take = std::min<int64_t>(cap[i], (int64_t)(c.pending.size() - c.pending_pos));
+		if (take > 0) memcpy(out[i], c.pending.data() + c.pending_pos, (size_t)take);
+		c.pending_pos += (size_t)take;
+		got[i] = take;
+		if (c.pending_pos == c.pending.size()) {
+			c.pending.clear();
+			c.pending_pos = 0;
+		}
+	}
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_check(b200z_deflate_streams *S, uint32_t *check) {
+	if (!S || (!S->s.empty() && !check)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	for (size_t i = 0; i < S->s.size(); i++) check[i] = S->wrap == B200Z_WRAP_RAW ? 0u : S->s[i].check;
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_stats(b200z_deflate_streams *S, int64_t *v, int32_t cap) {
+	if (!S || cap < 0 || (cap > 0 && !v)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	for (int32_t i = 0; i < cap && i < 4; i++) v[i] = S->stats[i];
+	return B200Z_OK;
+}
+
+int b200z_deflate_streams_destroy(b200z_deflate_streams *S) {
+	if (!S) return B200Z_OK;
+	DeviceGuard guard(S->device); // (the device buffers go while the set's device is current)
+	if (S->cs) {
+		cudaStreamSynchronize(S->cs);
+		cudaStreamDestroy(S->cs);
+	}
+	delete S;
 	return B200Z_OK;
 }
 
