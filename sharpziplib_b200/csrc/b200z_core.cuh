@@ -41,7 +41,9 @@ constexpr int kMaxDist = kWSize - (kMaxMatch + kMinMatch + 1); // 32506, Deflate
 constexpr int kTooFar = 4096;                                  // DeflaterEngine.cs:51
 constexpr int kBlockSyms = 16384;                              // DeflaterHuffman.BUFSIZE, DeflaterHuffman.cs:15
 constexpr int kLiteralNum = 286, kDistNum = 30, kBitlenNum = 19;
-constexpr int kTreeScratchInts = 10 * 286;
+// build_tree's scratch for a tree of n symbols (18 * n + 3 bytes, see there), and for the literal tree
+B200Z_HD constexpr int tree_scratch_ints(int n) { return (9 * n + 3) / 2 + 2; }
+constexpr int kTreeScratchInts = tree_scratch_ints(kLiteralNum);
 constexpr int kHdrWords = 160; // dynamic header: <= 17 + 57 + 316 * 14 bits = 4498 bits < 160 * 32
 constexpr uint32_t kSlideFirst = 65273; // first input offset whose window index reaches 65274 (trap T8)
 
@@ -738,22 +740,27 @@ inline void stored_run(uint32_t n, uint32_t dict_len, int end_mode, BlockFn bloc
 }
 
 // ---- DeflaterHuffman.cs helpers ----------------------------------------------------------------
-B200Z_HD int lcode(int len_m3) { // Lcode :932-946 (argument is length - 3)
-	if (len_m3 == 255) return 285;
-	int code = 257;
-	while (len_m3 >= 8) {
-		code += 4;
-		len_m3 >>= 1;
-	}
-	return code + len_m3;
+// floor(log2(x)) for x > 0
+B200Z_HD int ilog2(uint32_t x) {
+#ifdef __CUDA_ARCH__
+	return 31 - __clz((int)x);
+#else
+	return 31 - __builtin_clz(x);
+#endif
 }
-B200Z_HD int dcode(int dist_m1) { // Dcode :948-957 (argument is distance - 1)
-	int code = 0;
-	while (dist_m1 >= 4) {
-		code += 2;
-		dist_m1 >>= 1;
-	}
-	return code + dist_m1;
+// Lcode :932-946 (argument is length - 3).  The reference halves len_m3 until it is below 8, adding 4 per halving: that is
+// ilog2(len_m3) - 2 halvings, in closed form so that the lanes of a warp do not diverge on the loop.
+B200Z_HD int lcode(int len_m3) {
+	if (len_m3 == 255) return 285;
+	if (len_m3 < 8) return 257 + len_m3;
+	const int k = ilog2((uint32_t)len_m3) - 2;
+	return 257 + 4 * k + (len_m3 >> k);
+}
+// Dcode :948-957 (argument is distance - 1): ilog2(dist_m1) - 1 halvings of 2 each, likewise
+B200Z_HD int dcode(int dist_m1) {
+	if (dist_m1 < 4) return dist_m1;
+	const int k = ilog2((uint32_t)dist_m1) - 1;
+	return 2 * k + (dist_m1 >> k);
 }
 B200Z_HD int lcode_extra_bits(int lc) { // CompressBlock :716-720
 	int bits = (lc - 261) / 4;
@@ -781,11 +788,18 @@ B200Z_HD uint32_t static_dcode(int i) { return bit_reverse16((uint32_t)i << 11);
 
 // Tree.BuildTree + BuildLength (DeflaterHuffman.cs:196-329, :475-579), operation for operation.
 //   freqs[numSymbols] in; length[numSymbols], bl_counts[maxLength], numCodes out.
-//   scratch: heap[numSymbols] + childs[4*L-2] + values[2*L-1] + lengths[2*L-1] ints with L <= numSymbols
-//            ->  9 * numSymbols ints, plus numSymbols for hval[] below (kTreeScratchInts for the 286-symbol literal tree).
+//   scratch (tree_scratch_ints(numSymbols) ints, 8-byte aligned): heap[numSymbols + 1] entries of (value, node), then childs[4*L-2]
+//   as 16-bit node numbers (< 2 * L - 1, or -1), then lengths[2*L-1] bytes (<= maxLength), with L <= numSymbols leaves.  The
+//   reference's values[] array is only ever written (the heap reads its copy), so it is not kept.
+// Each heap entry holds its node's value next to the node number, so that a heap step reads and writes one 8-byte entry
+// per child: the tree is built by a single thread, its time is the sum of these load latencies, and with many CTAs on an
+// SM the shared-memory instructions of all their tree builds share one pipe.
+struct alignas(8) HeapEnt {
+	int32_t val, node;
+};
 B200Z_HDN int build_tree(const int *freqs, int numSymbols, int minNumCodes, int maxLength, uint8_t *length,
                          int *bl_counts, int *scratch) {
-	int *heap = scratch;
+	HeapEnt *heap = reinterpret_cast<HeapEnt *>(scratch);
 	int heapLen = 0;
 	int maxCode = 0;
 	for (int n = 0; n < numSymbols; n++) {
@@ -793,92 +807,72 @@ B200Z_HDN int build_tree(const int *freqs, int numSymbols, int minNumCodes, int 
 		if (freq != 0) {
 			int pos = heapLen++;
 			int ppos;
-			while (pos > 0 && freqs[heap[ppos = (pos - 1) / 2]] > freq) {
-				heap[pos] = heap[ppos];
+			while (pos > 0 && freqs[heap[ppos = (pos - 1) / 2].node] > freq) {
+				heap[pos].node = heap[ppos].node;
 				pos = ppos;
 			}
-			heap[pos] = n;
+			heap[pos].node = n;
 			maxCode = n;
 		}
 	}
 	while (heapLen < 2) {
 		int node = maxCode < 2 ? ++maxCode : 0;
-		heap[heapLen++] = node;
+		heap[heapLen++].node = node;
 	}
 	int numCodes = (maxCode + 1 > minNumCodes) ? maxCode + 1 : minNumCodes;
 	int numLeafs = heapLen;
-	int *childs = scratch + numSymbols;            // 4*heapLen - 2
-	int *values = childs + (4 * numLeafs - 2);     // 2*heapLen - 1
-	int *lengths = values + (2 * numLeafs - 1);    // 2*heapLen - 1
-	// hval[i] caches values[heap[i]] (always kept equal), so that a heap comparison is one load instead of two dependent
-	// ones -- the tree is built by a single thread and its time is the sum of these load latencies
-	int *hval = scratch + 9 * numSymbols;
+	int16_t *childs = reinterpret_cast<int16_t *>(heap + numSymbols + 1);       // 4*heapLen - 2
+	uint8_t *lengths = reinterpret_cast<uint8_t *>(childs + (4 * numLeafs - 2)); // 2*heapLen - 1
 	int numNodes = numLeafs;
 	for (int i = 0; i < heapLen; i++) {
-		int node = heap[i];
-		childs[2 * i] = node;
+		int node = heap[i].node;
+		childs[2 * i] = (int16_t)node;
 		childs[2 * i + 1] = -1;
-		values[i] = hval[i] = freqs[node] << 8;
-		heap[i] = i;
+		heap[i] = HeapEnt{freqs[node] << 8, i};
 	}
+	// heap[heapLen] is kept above every value: a node whose right child would be heap[heapLen] then takes its left child, as
+	// the reference's "path + 1 < heapLen" test decides, without the test
+	heap[heapLen] = HeapEnt{0x7FFFFFFF, -1};
 	do {
-		int first = heap[0];
-		int firstVal = hval[0];
-		int last = heap[--heapLen];
-		int lastVal = hval[heapLen];
+		const HeapEnt top = heap[0];
+		const int first = top.node, firstVal = top.val;
+		const HeapEnt bottom = heap[--heapLen];
+		heap[heapLen].val = 0x7FFFFFFF;
+		int last = bottom.node;
+		int lastVal = bottom.val;
 		int ppos = 0;
 		int path = 1;
 		while (path < heapLen) {
 			// both children are fetched before the comparison decides
-			const int v0 = hval[path], h0 = heap[path];
-			int v1 = 0, h1 = 0;
-			if (path + 1 < heapLen) {
-				v1 = hval[path + 1];
-				h1 = heap[path + 1];
-			}
-			const bool right = path + 1 < heapLen && v0 > v1;
+			const HeapEnt e0 = heap[path], e1 = heap[path + 1];
+			const bool right = e0.val > e1.val;
 			if (right) path++;
-			heap[ppos] = right ? h1 : h0;
-			hval[ppos] = right ? v1 : v0;
+			heap[ppos] = right ? e1 : e0;
 			ppos = path;
 			path = path * 2 + 1;
 		}
-		while ((path = ppos) > 0 && hval[ppos = (path - 1) / 2] > lastVal) {
-			heap[path] = heap[ppos];
-			hval[path] = hval[ppos];
-		}
-		heap[path] = last;
-		hval[path] = lastVal;
-		int second = heap[0];
-		int secondVal = hval[0];
+		while ((path = ppos) > 0 && heap[ppos = (path - 1) / 2].val > lastVal) heap[path] = heap[ppos];
+		heap[path] = HeapEnt{lastVal, last};
+		const HeapEnt sec = heap[0];
+		const int second = sec.node, secondVal = sec.val;
 		last = numNodes++;
-		childs[2 * last] = first;
-		childs[2 * last + 1] = second;
+		childs[2 * last] = (int16_t)first;
+		childs[2 * last + 1] = (int16_t)second;
 		int d1 = firstVal & 0xff, d2 = secondVal & 0xff;
 		int mindepth = d1 < d2 ? d1 : d2;
-		values[last] = lastVal = firstVal + secondVal - mindepth + 1;
+		lastVal = firstVal + secondVal - mindepth + 1;
 		ppos = 0;
 		path = 1;
 		while (path < heapLen) {
-			const int v0 = hval[path], h0 = heap[path];
-			int v1 = 0, h1 = 0;
-			if (path + 1 < heapLen) {
-				v1 = hval[path + 1];
-				h1 = heap[path + 1];
-			}
-			const bool right = path + 1 < heapLen && v0 > v1;
+			const HeapEnt e0 = heap[path], e1 = heap[path + 1];
+			const bool right = e0.val > e1.val;
 			if (right) path++;
-			heap[ppos] = right ? h1 : h0;
-			hval[ppos] = right ? v1 : v0;
+			heap[ppos] = right ? e1 : e0;
 			ppos = path;
 			path = ppos * 2 + 1;
 		}
-		while ((path = ppos) > 0 && hval[ppos = (path - 1) / 2] > lastVal) {
-			heap[path] = heap[ppos];
-			hval[path] = hval[ppos];
-		}
-		heap[path] = last;
-		hval[path] = lastVal;
+		while ((path = ppos) > 0 && heap[ppos = (path - 1) / 2].val > lastVal) heap[path] = heap[ppos];
+		heap[path] = HeapEnt{lastVal, last};
 	} while (heapLen > 1);
 
 	// BuildLength (:475-579); childs.Length / 2 == numNodes == 2 * numLeafs - 1
@@ -893,7 +887,7 @@ B200Z_HDN int build_tree(const int *freqs, int numSymbols, int minNumCodes, int 
 				bitLength = maxLength;
 				overflow++;
 			}
-			lengths[childs[2 * i]] = lengths[childs[2 * i + 1]] = bitLength;
+			lengths[childs[2 * i]] = lengths[childs[2 * i + 1]] = (uint8_t)bitLength;
 		} else {
 			int bitLength = lengths[i];
 			bl_counts[bitLength - 1]++;
@@ -966,34 +960,22 @@ struct BitCounter {
 
 // Tree.CalcBLFreq (:349-405) and Tree.WriteTree (:411-473) share one run-length walk; Sink decides what a
 // visit does.  visit(symbol) for a bit-length symbol, extra(value, bits) for the repeat counts.
+// The walk's steps never cross from one run of equal code lengths into the next (its inner loop stops at the first
+// different length, and the first step of a run of a nonzero length always sees curlen != nextlen), so what a run emits
+// depends on its length value and its size alone: walk_code_run() is that, and k_plan runs it for all runs at once.
 template <class Visit, class Extra>
-B200Z_HD void walk_code_lengths(const uint8_t *length, int numCodes, Visit visit, Extra extra) {
-	int max_count, min_count, count;
-	int curlen = -1;
-	int i = 0;
-	while (i < numCodes) {
-		count = 1;
-		int nextlen = length[i];
-		if (nextlen == 0) {
-			max_count = 138;
-			min_count = 3;
-		} else {
-			max_count = 6;
-			min_count = 3;
-			if (curlen != nextlen) {
-				visit(nextlen);
-				count = 0;
-			}
-		}
-		curlen = nextlen;
-		i++;
-		while (i < numCodes && curlen == length[i]) {
-			i++;
-			if (++count >= max_count) break;
-		}
-		if (count < min_count) {
-			while (count-- > 0) visit(curlen);
-		} else if (curlen != 0) {
+B200Z_HD void walk_code_run(int len, int run, Visit visit, Extra extra) {
+	const int max_count = len == 0 ? 138 : 6;
+	if (len != 0) {
+		visit(len);
+		run--;
+	}
+	while (run > 0) {
+		const int count = run < max_count ? run : max_count;
+		run -= count;
+		if (count < 3) {
+			for (int k = 0; k < count; k++) visit(len);
+		} else if (len != 0) {
 			visit(16);
 			extra(count - 3, 2);
 		} else if (count <= 10) {
@@ -1004,6 +986,29 @@ B200Z_HD void walk_code_lengths(const uint8_t *length, int numCodes, Visit visit
 			extra(count - 11, 7);
 		}
 	}
+}
+template <class Visit, class Extra>
+B200Z_HD void walk_code_lengths(const uint8_t *length, int numCodes, Visit visit, Extra extra) {
+	int i = 0;
+	while (i < numCodes) {
+		int j = i + 1;
+		while (j < numCodes && length[j] == length[i]) j++;
+		walk_code_run(length[i], j - i, visit, extra);
+		i = j;
+	}
+}
+
+// BL_ORDER (DeflaterHuffman.cs:33): the order in which the bit-length code lengths are sent
+B200Z_HD int bl_order(int i) {
+	if (i < 3) return 16 + i;
+	if (i == 3) return 0;
+	return (i & 1) ? 7 - ((i - 5) >> 1) : 8 + ((i - 4) >> 1);
+}
+// FlushBlock's choice (:830-857) from opt_len (dynamic trees, header included) and static_len: 0 stored, 1 static, 2 dynamic
+B200Z_HD int block_type(int stored_ok, int storedLength, int opt_len, int static_len) {
+	if (opt_len >= static_len) opt_len = static_len; // force static trees
+	if (stored_ok && storedLength + 4 < (opt_len >> 3)) return 0;
+	return opt_len == static_len ? 1 : 2;
 }
 
 // Everything FlushBlock (:788-857) decides for one block, from its histograms.
@@ -1018,8 +1023,8 @@ struct BlockPlan {
 // freqs are the literal (286) and distance (30) histograms with EOB already counted; extra_bits as tallied by
 // TallyDist (:894-916).  Outputs code lengths / codes for the block's chosen trees and, for dynamic blocks, the
 // header bit string into hdr_words (zeroed by the caller, >= kHdrWords words).  scratch >= kTreeScratchInts ints.
-// plan_block() = build_tree(lit) + build_tree(dist) + plan_block_finish(); the kernel runs the two tree builds on two
-// threads at once and then calls plan_block_finish() on one of them.
+// plan_block() = build_tree(lit) + build_tree(dist) + plan_block_finish(), serially; k_plan runs the same steps with the
+// order-free ones spread over its warps.
 B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, int extra_bits, int stored_ok, int storedLength,
                                  int lastBlock, int lit_nc, const int *lit_blc, int dist_nc, const int *dist_blc, uint8_t *lit_len,
                                  uint16_t *lit_codes, uint8_t *dist_len, uint16_t *dist_codes, uint32_t *hdr_words, int *scratch,
@@ -1039,7 +1044,6 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
                                  int lastBlock, int lit_nc, const int *lit_blc, int dist_nc, const int *dist_blc, uint8_t *lit_len,
                                  uint16_t *lit_codes, uint8_t *dist_len, uint16_t *dist_codes, uint32_t *hdr_words, int *scratch,
                                  BlockPlan &plan) {
-	const int BL_ORDER[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 	int bl_blc[7];
 	int bl_freqs[kBitlenNum];
 	uint8_t bl_len[kBitlenNum];
@@ -1050,7 +1054,7 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
 	build_tree(bl_freqs, kBitlenNum, 4, 7, bl_len, bl_blc, scratch);
 	int blTreeCodes = 4;
 	for (int i = 18; i > blTreeCodes; i--) {
-		if (bl_len[BL_ORDER[i]] > 0) blTreeCodes = i + 1;
+		if (bl_len[bl_order(i)] > 0) blTreeCodes = i + 1;
 	}
 	int opt_len = 14 + blTreeCodes * 3 + extra_bits;
 	for (int i = 0; i < kBitlenNum; i++) opt_len += bl_freqs[i] * bl_len[i];
@@ -1063,16 +1067,14 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
 	plan.dist_numCodes = dist_nc;
 	plan.blTreeCodes = blTreeCodes;
 	plan.static_len = static_len;
-	int dyn_len = opt_len;
-	if (opt_len >= static_len) opt_len = static_len; // force static trees
+	plan.type = block_type(stored_ok, storedLength, opt_len, static_len);
+	if (opt_len >= static_len) opt_len = static_len;
 	plan.opt_len = opt_len;
-	if (stored_ok && storedLength + 4 < (opt_len >> 3)) {
-		plan.type = 0;
+	if (plan.type == 0) {
 		plan.hdr_bits = 3;
 		plan.body_bits = 0;
 		hdr_words[0] = (uint32_t)((0 << 1) + (lastBlock ? 1 : 0));
-	} else if (opt_len == static_len) {
-		plan.type = 1;
+	} else if (plan.type == 1) {
 		plan.hdr_bits = 3;
 		plan.body_bits = (uint32_t)static_len;
 		hdr_words[0] = (uint32_t)((1 << 1) + (lastBlock ? 1 : 0));
@@ -1085,7 +1087,6 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
 			dist_codes[i] = (uint16_t)static_dcode(i);
 		}
 	} else {
-		plan.type = 2;
 		// SendAllTrees (:676-696)
 		build_codes(bl_len, bl_blc, 7, kBitlenNum, bl_codes); // blTree.numCodes is irrelevant: all 19 get codes
 		build_codes(lit_len, lit_blc, 15, lit_nc, lit_codes);
@@ -1095,7 +1096,7 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
 		sink.put((uint32_t)(lit_nc - 257), 5);
 		sink.put((uint32_t)(dist_nc - 1), 5);
 		sink.put((uint32_t)(blTreeCodes - 4), 4);
-		for (int rank = 0; rank < blTreeCodes; rank++) sink.put(bl_len[BL_ORDER[rank]], 3);
+		for (int rank = 0; rank < blTreeCodes; rank++) sink.put(bl_len[bl_order(rank)], 3);
 		walk_code_lengths(lit_len, lit_nc, [&](int s) { sink.put(bl_codes[s], bl_len[s]); },
 		                  [&](int v, int nb) { sink.put((uint32_t)v, nb); });
 		walk_code_lengths(dist_len, dist_nc, [&](int s) { sink.put(bl_codes[s], bl_len[s]); },
@@ -1106,7 +1107,6 @@ B200Z_HDN void plan_block_finish(const int *lit_freqs, const int *dist_freqs, in
 		for (int i = 0; i < kLiteralNum; i++) body += lit_freqs[i] * lit_len[i];
 		for (int i = 0; i < kDistNum; i++) body += dist_freqs[i] * dist_len[i];
 		plan.body_bits = (uint32_t)body;
-		(void)dyn_len;
 	}
 }
 

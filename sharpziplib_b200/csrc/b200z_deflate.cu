@@ -1350,41 +1350,95 @@ __global__ void k_set_results(int n, const int64_t *__restrict__ lens, int64_t *
 
 // ------------------------------------------------------------------------------------------------
 // K4: per-block histograms, the reference's Huffman construction and the block type decision.
+// One CTA of two warps per block.  Only the heap of each Tree.BuildTree and BuildLength (whose tie-breaks decide the
+// bytes) run on one lane, the literal and the distance tree on one lane of each warp; everything around them is
+// order-free and runs warp-wide: the histogram, CalcBLFreq and the header's code-length string (per run of equal code
+// lengths, walk_code_run), the cost sums and BuildCodes.  What plan_block_finish() does serially for the CPU model.
+// The footprint (8.3 KiB of shared memory, <= 40 registers, no stack frame) keeps 24 CTAs on an SM: the 7,213 blocks of
+// bench.py's 1024 x 256 KiB at level 6 run in 2.3 waves of 3,168 CTAs on an H100.
 // ------------------------------------------------------------------------------------------------
 constexpr int kPlanThreads = 64;
-__global__ void __launch_bounds__(kPlanThreads)
+
+__device__ __forceinline__ uint32_t lanes_below() {
+	return (1u << (threadIdx.x & 31)) - 1u;
+}
+__device__ __forceinline__ void or_hdr(uint32_t *w, uint32_t pos, uint32_t v, int count) {
+	const uint32_t idx = pos >> 5, sh = pos & 31;
+	atomicOr(w + idx, v << sh);
+	if (sh + (uint32_t)count > 32) atomicOr(w + idx + 1, v >> (32 - sh));
+}
+// Tree.BuildCodes warp-wide: symbol i gets nextCode[len] + (the symbols in front of it with the same length) << (16 - len).
+// next[0..maxLength) is the per-length start from the bl_counts, advanced chunk by chunk.
+__device__ void build_codes_warp(const uint8_t *length, const int *bl_counts, int maxLength, int numCodes, uint16_t *codes,
+                                 int *next) {
+	const int lane = threadIdx.x & 31;
+	if (lane == 0) {
+		int code = 0;
+		for (int bits = 0; bits < maxLength; bits++) {
+			next[bits] = code;
+			code += bl_counts[bits] << (15 - bits);
+		}
+	}
+	__syncwarp();
+	for (int base = 0; base < numCodes; base += 32) {
+		const int i = base + lane;
+		const int bits = i < numCodes ? length[i] : 0;
+		const uint32_t peers = __match_any_sync(0xffffffffu, bits);
+		if (i < numCodes)
+			codes[i] = bits ? (uint16_t)bit_reverse16((uint32_t)(next[bits - 1] + (__popc(peers & lanes_below()) << (16 - bits)))) : 0;
+		__syncwarp();
+		if (bits && (peers >> lane) == 1u) next[bits - 1] += __popc(peers) << (16 - bits); // the group's last lane
+		__syncwarp();
+	}
+}
+// sum over a warp
+__device__ __forceinline__ int warp_sum(int v) {
+	for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+	return v;
+}
+
+__global__ void __launch_bounds__(kPlanThreads, 24)
     k_plan(const uint32_t *__restrict__ sym, const int64_t *__restrict__ in_off, const int64_t *__restrict__ in_len,
            const uint32_t *__restrict__ nsyms, const uint32_t *__restrict__ nblocks, const uint32_t *__restrict__ blk_off,
            const int32_t *__restrict__ blk_desc, const uint32_t *__restrict__ blk_start, const uint32_t *__restrict__ blk_ptop,
            BlockMeta *__restrict__ meta, BlockTables *__restrict__ tables, const int64_t *__restrict__ bias, int end_mode) {
 	__shared__ int s_lit[kLiteralNum];
 	__shared__ int s_dist[kDistNum];
-	__shared__ int s_extra;
-	__shared__ int s_scratch[kTreeScratchInts];
-	__shared__ int s_scratch2[10 * kDistNum];
-	__shared__ int s_lit_blc[15], s_dist_blc[15], s_nc[2];
-	__shared__ BlockTables s_tab;
+	__align__(8) __shared__ int s_scratch[tree_scratch_ints(kLiteralNum)]; // the literal tree, then the header and the runs
+	__align__(8) __shared__ int s_scratch2[tree_scratch_ints(kDistNum)];   // the distance tree, then the bit-length tree
+	__shared__ int s_blc[3][16];  // bl_counts of the literal, distance and bit-length trees
+	__shared__ int s_next[3][16]; // BuildCodes' nextCode, per tree
+	__shared__ int s_bl_freqs[kBitlenNum];
+	__shared__ uint8_t s_bl_len[kBitlenNum + 1];
+	__shared__ uint16_t s_bl_codes[kBitlenNum + 1];
+	__shared__ int s_v[6]; // extra bits, literal numCodes, distance numCodes, static_len, dynamic body bits, runs
+	// the members of BlockTables in front of hdr (the header words live in s_scratch, where the literal tree was built);
+	// s_tab.hdr is never touched
+	__align__(16) __shared__ uint8_t s_tabmem[offsetof(BlockTables, hdr)];
+	BlockTables &s_tab = *reinterpret_cast<BlockTables *>(s_tabmem);
+	uint32_t *hdr = reinterpret_cast<uint32_t *>(s_scratch);
 	const int g = blockIdx.x;
 	const int stream = blk_desc[g];
 	const uint32_t b = (uint32_t)g - blk_off[stream];
 	const uint32_t nb = nblocks[stream];
 	if (b >= nb) return;
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const uint32_t ns = nsyms[stream];
 	const uint32_t s0 = b * (uint32_t)kBlockSyms;
 	const uint32_t s1 = (ns - s0 > (uint32_t)kBlockSyms) ? s0 + kBlockSyms : ns;
 	const uint32_t *sp = sym + in_off[stream];
-	for (int i = threadIdx.x; i < kLiteralNum; i += blockDim.x) s_lit[i] = 0;
-	for (int i = threadIdx.x; i < kDistNum; i += blockDim.x) s_dist[i] = 0;
-	for (int i = threadIdx.x; i < kHdrWords; i += blockDim.x) s_tab.hdr[i] = 0;
-	if (threadIdx.x == 0) s_extra = 0;
+	for (int i = tid; i < kLiteralNum; i += kPlanThreads) s_lit[i] = 0;
+	for (int i = tid; i < kDistNum; i += kPlanThreads) s_dist[i] = 0;
+	if (tid < kBitlenNum) s_bl_freqs[tid] = 0;
+	if (tid == 0) s_v[0] = 0;
 	__syncthreads();
 	int extra = 0;
-	for (uint32_t i0 = s0 + threadIdx.x; i0 < s1; i0 += 8 * blockDim.x) {
+	for (uint32_t i0 = s0 + tid; i0 < s1; i0 += 8 * kPlanThreads) {
 		// eight independent loads in flight per thread (ncu: the one-load-per-trip loop sat on long_scoreboard)
 		uint32_t sv[8];
 #pragma unroll
 		for (int k = 0; k < 8; k++) {
-			const uint32_t i = i0 + (uint32_t)k * blockDim.x;
+			const uint32_t i = i0 + (uint32_t)k * kPlanThreads;
 			sv[k] = i < s1 ? __ldg(sp + i) : 0xFFFFFFFFu;
 		}
 #pragma unroll
@@ -1401,45 +1455,164 @@ __global__ void __launch_bounds__(kPlanThreads)
 			}
 		}
 	}
-	for (int o = 16; o > 0; o >>= 1) extra += __shfl_down_sync(0xffffffffu, extra, o);
-	if ((threadIdx.x & 31) == 0 && extra) atomicAdd(&s_extra, extra);
+	extra = warp_sum(extra);
+	if (lane == 0 && extra) atomicAdd(&s_v[0], extra);
 	__syncthreads();
-	if (threadIdx.x == 0) s_lit[256] += 1; // FlushBlock: literalTree.freqs[EOF_SYMBOL]++ (:790)
+	if (tid == 0) s_lit[256] += 1; // FlushBlock: literalTree.freqs[EOF_SYMBOL]++ (:790)
 	__syncthreads();
 	// the two big trees are independent: build them on two warps at once
-	if (threadIdx.x == 0) s_nc[0] = build_tree(s_lit, kLiteralNum, 257, 15, s_tab.lit_len, s_lit_blc, s_scratch);
-	if (threadIdx.x == 32) s_nc[1] = build_tree(s_dist, kDistNum, 1, 15, s_tab.dist_len, s_dist_blc, s_scratch2);
+	if (tid == 0) s_v[1] = build_tree(s_lit, kLiteralNum, 257, 15, s_tab.lit_len, s_blc[0], s_scratch);
+	if (tid == 32) s_v[2] = build_tree(s_dist, kDistNum, 1, 15, s_tab.dist_len, s_blc[1], s_scratch2);
 	__syncthreads();
-	if (threadIdx.x == 0) {
-		const uint32_t *bstart = blk_start + blk_off[stream];
-		const uint32_t *bptop = blk_ptop + blk_off[stream];
-		const uint32_t byte_start = bstart[b];
-		const uint32_t n = (uint32_t)in_len[stream];
-		// (an open run's last written block ends at a cut, like every block in front of it)
-		const uint32_t byte_len = ((b + 1 < nb || end_mode == B200Z_END_NONE) ? bstart[b + 1] : n) - byte_start;
-		// storedOffset is window relative and goes negative once the block start has been slid out (trap T4)
-		const long long ab = bias[stream]; // absolute stream offset of buffer position 0
-		long long storedOffset = (long long)byte_start + ab + 1 - 32768ll * (long long)slides_done((uint32_t)(bptop[b] + ab));
-		if (bptop[b] >= 0xFFFFFFFEu) storedOffset = bptop[b] == 0xFFFFFFFEu ? 0 : -1; // levels 1-4: decided by k_fast
-		const int last = (b + 1 == nb) && end_mode == B200Z_END_FINISH;
-		BlockPlan plan;
-		plan_block_finish(s_lit, s_dist, s_extra, storedOffset >= 0, (int)byte_len, last, s_nc[0], s_lit_blc, s_nc[1], s_dist_blc,
-		                  s_tab.lit_len, s_tab.lit_codes, s_tab.dist_len, s_tab.dist_codes, s_tab.hdr, s_scratch, plan);
+	const int lit_nc = s_v[1], dist_nc = s_v[2], nlen = lit_nc + dist_nc;
+	uint16_t *runs = reinterpret_cast<uint16_t *>(hdr + kHdrWords); // first code length of every run, then nlen
+	auto len_at = [&](int j) -> int { return j < lit_nc ? s_tab.lit_len[j] : s_tab.dist_len[j - lit_nc]; };
+	if (warp == 0) {
+		// CalcBLFreq: the runs of equal code lengths (the walk restarts at the distance lengths), then their symbols
+		int nruns = 0;
+		for (int base = 0; base < nlen; base += 32) {
+			const int j = base + lane;
+			const bool start = j < nlen && (j == 0 || j == lit_nc || len_at(j) != len_at(j - 1));
+			const uint32_t m = __ballot_sync(0xffffffffu, start);
+			if (start) runs[nruns + __popc(m & lanes_below())] = (uint16_t)j;
+			nruns += __popc(m);
+		}
+		if (lane == 0) {
+			runs[nruns] = (uint16_t)nlen;
+			s_v[5] = nruns;
+		}
+		__syncwarp();
+		for (int k = lane; k < nruns; k += 32)
+			walk_code_run(len_at(runs[k]), runs[k + 1] - runs[k], [&](int s) { atomicAdd(&s_bl_freqs[s], 1); }, [](int, int) {});
+	} else {
+		// the cost sums that do not need the bit-length tree
+		int st = 0, dyn = 0;
+		for (int i = lane; i < kLiteralNum; i += 32) {
+			st += s_lit[i] * static_llen(i);
+			dyn += s_lit[i] * s_tab.lit_len[i];
+		}
+		if (lane < kDistNum) {
+			st += s_dist[lane] * 5;
+			dyn += s_dist[lane] * s_tab.dist_len[lane];
+		}
+		st = warp_sum(st);
+		dyn = warp_sum(dyn);
+		if (lane == 0) {
+			s_v[3] = s_v[0] + st;
+			s_v[4] = s_v[0] + dyn;
+		}
+		for (int i = lane; i < kHdrWords; i += 32) hdr[i] = 0;
+	}
+	__syncthreads();
+	if (tid == 0) build_tree(s_bl_freqs, kBitlenNum, 4, 7, s_bl_len, s_blc[2], s_scratch2);
+	__syncthreads();
+	int blTreeCodes = 4;
+	for (int i = 18; i > blTreeCodes; i--) {
+		if (s_bl_len[bl_order(i)] > 0) blTreeCodes = i + 1;
+	}
+	int bl_cost = 0;
+	for (int i = 0; i < kBitlenNum; i++) bl_cost += s_bl_freqs[i] * s_bl_len[i];
+	const int static_len = s_v[3], body = s_v[4];
+	int opt_len = 14 + blTreeCodes * 3 + bl_cost + body;
+	if (opt_len >= static_len) opt_len = static_len; // force static trees
+
+	const uint32_t *bstart = blk_start + blk_off[stream];
+	const uint32_t byte_start = bstart[b];
+	const uint32_t n = (uint32_t)in_len[stream];
+	// (an open run's last written block ends at a cut, like every block in front of it)
+	const uint32_t byte_len = ((b + 1 < nb || end_mode == B200Z_END_NONE) ? bstart[b + 1] : n) - byte_start;
+	// storedOffset is window relative and goes negative once the block start has been slid out (trap T4)
+	const uint32_t ptop = blk_ptop[blk_off[stream] + b];
+	const long long ab = bias[stream]; // absolute stream offset of buffer position 0
+	long long storedOffset = (long long)byte_start + ab + 1 - 32768ll * (long long)slides_done((uint32_t)(ptop + ab));
+	if (ptop >= 0xFFFFFFFEu) storedOffset = ptop == 0xFFFFFFFEu ? 0 : -1; // levels 1-4: decided by k_fast
+	const int last = (b + 1 == nb) && end_mode == B200Z_END_FINISH;
+	const int type = block_type(storedOffset >= 0, (int)byte_len, opt_len, static_len);
+	uint32_t hdr_bits = 3, body_bits = 0;
+	if (type == 0) {
+		if (tid == 0) hdr[0] = (uint32_t)((0 << 1) + last);
+	} else if (type == 1) {
+		body_bits = (uint32_t)static_len;
+		if (tid == 0) hdr[0] = (uint32_t)((1 << 1) + last);
+		for (int i = tid; i < kLiteralNum; i += kPlanThreads) {
+			s_tab.lit_len[i] = (uint8_t)static_llen(i);
+			s_tab.lit_codes[i] = (uint16_t)static_lcode(i);
+		}
+		if (tid < kDistNum) {
+			s_tab.dist_len[tid] = 5;
+			s_tab.dist_codes[tid] = (uint16_t)static_dcode(tid);
+		}
+	} else {
+		// SendAllTrees (:676-696)
+		body_bits = (uint32_t)body;
+		if (warp == 0) {
+			build_codes_warp(s_tab.lit_len, s_blc[0], 15, lit_nc, s_tab.lit_codes, s_next[0]);
+		} else {
+			build_codes_warp(s_tab.dist_len, s_blc[1], 15, dist_nc, s_tab.dist_codes, s_next[1]);
+			build_codes_warp(s_bl_len, s_blc[2], 7, kBitlenNum, s_bl_codes, s_next[2]);
+		}
+		__syncthreads();
+		const uint32_t pre = 17 + 3 * (uint32_t)blTreeCodes;
+		if (warp == 0) {
+			// the code-length string: every run's bits at its prefix-summed offset
+			const int nruns = s_v[5];
+			uint32_t off = pre;
+			for (int base = 0; base < nruns; base += 32) {
+				const int k = base + lane;
+				int v = 0, r = 0;
+				uint32_t nbits = 0;
+				if (k < nruns) {
+					v = len_at(runs[k]);
+					r = runs[k + 1] - runs[k];
+					walk_code_run(v, r, [&](int s) { nbits += s_bl_len[s]; }, [&](int, int nb) { nbits += (uint32_t)nb; });
+				}
+				uint32_t incl = nbits;
+				for (int o = 1; o < 32; o <<= 1) {
+					const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+					if (lane >= o) incl += t;
+				}
+				uint32_t pos = off + incl - nbits;
+				if (k < nruns)
+					walk_code_run(
+					    v, r,
+					    [&](int s) {
+						    or_hdr(hdr, pos, s_bl_codes[s], s_bl_len[s]);
+						    pos += s_bl_len[s];
+					    },
+					    [&](int x, int nb) {
+						    or_hdr(hdr, pos, (uint32_t)x, nb);
+						    pos += (uint32_t)nb;
+					    });
+				off += __shfl_sync(0xffffffffu, incl, 31);
+			}
+			hdr_bits = off;
+		} else {
+			if (lane == 0)
+				or_hdr(hdr, 0,
+				       (uint32_t)((2 << 1) + last) | (uint32_t)(lit_nc - 257) << 3 | (uint32_t)(dist_nc - 1) << 8 |
+				           (uint32_t)(blTreeCodes - 4) << 13,
+				       17);
+			if (lane < blTreeCodes) or_hdr(hdr, 17 + 3 * (uint32_t)lane, s_bl_len[bl_order(lane)], 3);
+		}
+	}
+	if (tid == 0) {
 		BlockMeta m;
 		m.byte_start = byte_start;
 		m.byte_len = byte_len;
 		m.nsyms = s1 - s0;
-		m.hdr_bits = plan.hdr_bits;
-		m.body_bits = plan.body_bits;
-		m.type = (uint32_t)plan.type;
+		m.hdr_bits = hdr_bits;
+		m.body_bits = body_bits;
+		m.type = (uint32_t)type;
 		m.bit_off = 0;
 		meta[g] = m;
 	}
 	__syncthreads();
-	// copy the tables out (16-byte vectors)
-	const uint4 *src = reinterpret_cast<const uint4 *>(&s_tab);
-	uint4 *dst = reinterpret_cast<uint4 *>(&tables[g]);
-	for (int i = threadIdx.x; i < (int)(sizeof(BlockTables) / 16); i += blockDim.x) dst[i] = src[i];
+	// copy the tables out
+	constexpr int kHdrOff = (int)offsetof(BlockTables, hdr) / 4;
+	static_assert(offsetof(BlockTables, hdr) % 4 == 0, "");
+	const uint32_t *src = reinterpret_cast<const uint32_t *>(s_tabmem);
+	uint32_t *dst = reinterpret_cast<uint32_t *>(&tables[g]);
+	for (int i = tid; i < kHdrOff + kHdrWords; i += kPlanThreads) dst[i] = i < kHdrOff ? src[i] : hdr[i - kHdrOff];
 }
 
 __device__ __forceinline__ void or_bits(uint32_t *out_words, uint64_t bitpos, uint64_t bits, int nbits) {
@@ -1972,6 +2145,7 @@ static int deflate_plan_build(DeflatePlan *p) {
 	B200Z_CUDA(cudaFuncSetAttribute(k_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_links, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinksSmem));
 	B200Z_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileData + 2 * 2 * kTile));
+	B200Z_CUDA(cudaFuncSetAttribute(k_plan, cudaFuncAttributePreferredSharedMemoryCarveout, 100)); // 24 CTAs per SM
 	return B200Z_OK;
 }
 
