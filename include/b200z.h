@@ -356,6 +356,49 @@ int b200z_deflate_streams_read(b200z_deflate_streams *s, uint8_t *const *out, co
 int b200z_deflate_streams_check(b200z_deflate_streams *s, uint32_t *check);
 int b200z_deflate_streams_stats(b200z_deflate_streams *s, int64_t *v, int32_t cap);
 int b200z_deflate_streams_destroy(b200z_deflate_streams *s);
+/* ---------------------------------------------------------------------------------------------------------------
+ * Inflater sets -- n independent Inflater streams that arrive in pieces (request bodies, zip entries, log shippers read
+ * as their bytes come in), decoded together: what N Inflater handles do, in one device pass per call.  Every stream
+ * keeps what the handle keeps between SetInput calls (its resume point, a copy of the current block's header, the
+ * compressed bytes from the resume point on); its window (the last 32 KiB of output) and running checksum stay on the
+ * device, so a write uploads the new compressed bytes and the few kept ones only.
+ * create: n streams of one wrap (RAW, ZLIB or RAW_CRC32; any other wrap, GZIP included, is B200Z_E_ARG), each as fresh
+ * as new Inflater(noHeader = wrap != ZLIB).  The set is bound to the device b200z_init chose for the calling thread;
+ * without a device B200Z_E_CUDA.
+ * write: per stream SetInput(in[i], len[i]) (len[i] = 0 is no call), then every stream with input it has not decoded and
+ * no dictionary awaited is decoded as far as its input goes, in plans on a CUDA stream of the set's own (each plan
+ * synchronises it twice).  Due streams are split into plans of at most 256 MiB of compressed and 4 GiB of output
+ * capacity; a stream whose output outgrows its capacity goes on from its resume point in a later plan of the same write.
+ * status[i] = code | detail << 8 as the plan statuses are: B200Z_OK once the stream has finished, B200Z_E_NEED_INPUT
+ * while it waits for input (no failure), its data error (the output in front of it stays readable; the stream takes no
+ * more input and keeps the status), or B200Z_E_STATE for input behind the end of a finished stream (that stream only;
+ * bytes behind the end in the write that finished it are kept as RemainingInput).  Returns the first status that is
+ * neither OK nor NEED_INPUT; b200z_last_error() names its stream and gives the reference's message.
+ * read: out[i] gets min(cap[i], undelivered) of what stream i has decoded, got[i] the count.  For every stream the
+ * concatenation of the reads is the reference Inflater's output for the same SetInput sequence.
+ * state (each array may be NULL): flags[i] bit 0 IsFinished (the end and, for ZLIB, a matching trailer), bit 1
+ * IsNeedingDictionary; total_in[i] TotalIn; total_out[i] the bytes decoded so far (TotalOut once they are read);
+ * remaining[i] RemainingInput (bytes behind the stream's end, trap T14); status[i] as write reports it.
+ * check: Inflater.Adler for ZLIB (the DICTID while a dictionary is awaited, else the Adler-32 of the output decoded so
+ * far), the CRC-32 of the output decoded so far for RAW_CRC32 (a zip entry's crc), 0 for RAW.
+ * set_dictionary: Inflater.SetDictionary (Inflater.cs:589-620) for stream i, with its errors ("Dictionary is not needed",
+ * "Wrong adler checksum"); the next write decodes what waited behind the header.
+ * stats: v[0] stream runs, v[1] plans run, v[2] plans created, v[3] the most compressed bytes one stream held at once,
+ * v[4] the most device workspace one plan took (bytes), v[5] host-to-device bytes the runs copied.  Plans are kept
+ * between writes and reused while the due streams fit them.
+ * detail_message: the reference's exception message for a status's detail.
+ * One set = one host thread at a time. */
+typedef struct b200z_inflate_streams b200z_inflate_streams;
+int b200z_inflate_streams_create(int32_t n, int wrap, b200z_inflate_streams **s);
+int b200z_inflate_streams_write(b200z_inflate_streams *s, const uint8_t *const *in, const int64_t *len, int32_t *status);
+int b200z_inflate_streams_read(b200z_inflate_streams *s, uint8_t *const *out, const int64_t *cap, int64_t *got);
+int b200z_inflate_streams_state(b200z_inflate_streams *s, int32_t *flags, int64_t *total_in, int64_t *total_out, int64_t *remaining,
+                                int32_t *status);
+int b200z_inflate_streams_check(b200z_inflate_streams *s, uint32_t *check);
+int b200z_inflate_streams_set_dictionary(b200z_inflate_streams *s, int32_t i, const uint8_t *dict, int32_t len);
+int b200z_inflate_streams_stats(b200z_inflate_streams *s, int64_t *v, int32_t cap);
+int b200z_inflate_streams_destroy(b200z_inflate_streams *s);
+const char *b200z_inflate_detail_message(int32_t status);
 
 /* worst-case compressed size for `len` input bytes at any level (capacity a caller should provide) */
 int64_t b200z_deflate_bound(int64_t len);

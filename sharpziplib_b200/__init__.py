@@ -9,6 +9,6 @@ from ._lib import (SharpZipBaseException, StreamDecodingException, B200zUnsuppor
 from .checksum import Crc32, Adler32, BZip2Crc  # noqa: F401
 from .codec import Deflater, Inflater, DeflateStrategy  # noqa: F401
 from .streams import DeflaterOutputStream, InflaterInputStream, GZipOutputStream, GZipInputStream  # noqa: F401
-from .batch import DeflatePlan, InflatePlan, Pipeline, DeflaterSet, deflate_batch, inflate_batch, zip_entries, unzip_entries  # noqa: F401
+from .batch import DeflatePlan, InflatePlan, Pipeline, DeflaterSet, InflaterSet, deflate_batch, inflate_batch, zip_entries, unzip_entries  # noqa: F401
 from .lzw import LzwException, LzwInputStream, LzwPlan, lzw_batch  # noqa: F401
 from . import encryption  # noqa: F401

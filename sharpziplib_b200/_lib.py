@@ -164,6 +164,15 @@ _SIGS = {
     "b200z_deflate_streams_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200z_deflate_streams_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "b200z_deflate_streams_destroy": (C.c_int, [C.c_void_p]),
+    "b200z_inflate_streams_create": (C.c_int, [C.c_int32, C.c_int, C.POINTER(C.c_void_p)]),
+    "b200z_inflate_streams_write": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_inflate_streams_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_inflate_streams_state": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_inflate_streams_check": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200z_inflate_streams_set_dictionary": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
+    "b200z_inflate_streams_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
+    "b200z_inflate_streams_destroy": (C.c_int, [C.c_void_p]),
+    "b200z_inflate_detail_message": (C.c_char_p, [C.c_int32]),
     "b200z_lzw_plan_create": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     "b200z_lzw_pipeline_create": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
     "b200z_lzw_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -342,6 +342,95 @@ class DeflaterSet:
     __del__ = close
 
 
+class InflaterSet:
+    """n independent Inflater streams of one wrap that arrive in pieces, decoded together on the device
+    (b200z_inflate_streams_*): what n Inflater objects behind InflaterInputStream do, with one device pass per write()
+    instead of one per stream.  wrap: WRAP_ZLIB, WRAP_RAW or WRAP_RAW_CRC32 (raw, with the CRC-32 a zip entry is checked
+    against)."""
+
+    def __init__(self, n, wrap=_lib.WRAP_ZLIB):
+        h = C.c_void_p()
+        _lib.raise_for(_lib.lib().b200z_inflate_streams_create(n, wrap, C.byref(h)))
+        self._h = h
+        self.n = n
+        self.status = np.zeros(n, dtype=np.int32)  # per stream, of the last write(): code | detail << 8
+        self._cap = np.full(n, 65536, dtype=np.int64)
+
+    def write(self, buffers):
+        """SetInput(buffers[i]) on every stream (an empty buffer is no call), then decode every stream as far as its input
+        goes.  A stream's data error is reported in status and errors(), not raised; input behind the end of a finished
+        stream makes its status E_STATE and raises InvalidOperationException after the other streams have gone on."""
+        if len(buffers) != self.n:
+            raise ValueError("one buffer per stream")
+        ins = [np.ascontiguousarray(np.frombuffer(b, dtype=np.uint8)) for b in buffers]
+        lens = np.array([a.size for a in ins], dtype=np.int64)
+        rc = _lib.lib().b200z_inflate_streams_write(self._h, _ptr_array(ins), lens.ctypes.data, self.status.ctypes.data)
+        codes = self.status & 0xFF
+        if rc != _lib.OK and (rc == _lib.E_STATE or not (codes == rc).any()):
+            _lib.raise_for(rc)  # a failure of the call, or input for a finished stream
+
+    def read(self):
+        """everything each stream has decoded since the last read(), as a list of bytes"""
+        parts = [[] for _ in range(self.n)]
+        want = np.ones(self.n, dtype=bool)
+        got = np.zeros(self.n, dtype=np.int64)
+        while want.any():
+            cap = np.where(want, self._cap, 0).astype(np.int64)
+            outs = [np.empty(int(c), dtype=np.uint8) for c in cap]
+            _lib.raise_for(_lib.lib().b200z_inflate_streams_read(self._h, _ptr_array(outs), cap.ctypes.data, got.ctypes.data))
+            for i in np.nonzero(want)[0]:
+                parts[i].append(outs[i][:got[i]].tobytes())
+            want &= got == cap
+            self._cap = np.where(want, np.minimum(self._cap * 4, 64 << 20), self._cap)
+        return [b"".join(p) for p in parts]
+
+    def state(self):
+        """per stream: {"finished", "needs_dictionary", "total_in", "total_out", "remaining", "status"}"""
+        fl = np.zeros(self.n, dtype=np.int32)
+        ti, to, rem = (np.zeros(self.n, dtype=np.int64) for _ in range(3))
+        st = np.zeros(self.n, dtype=np.int32)
+        _lib.raise_for(_lib.lib().b200z_inflate_streams_state(self._h, fl.ctypes.data, ti.ctypes.data, to.ctypes.data,
+                                                               rem.ctypes.data, st.ctypes.data))
+        return [{"finished": bool(fl[i] & 1), "needs_dictionary": bool(fl[i] & 2), "total_in": int(ti[i]),
+                 "total_out": int(to[i]), "remaining": int(rem[i]), "status": int(st[i])} for i in range(self.n)]
+
+    def checks(self):
+        """per stream: Inflater.Adler (WRAP_ZLIB) or the CRC-32 (WRAP_RAW_CRC32) of the output decoded so far; 0 for raw"""
+        v = np.zeros(self.n, dtype=np.uint32)
+        _lib.raise_for(_lib.lib().b200z_inflate_streams_check(self._h, v.ctypes.data))
+        return [int(x) for x in v]
+
+    def errors(self):
+        """per stream: None, or the reference's exception message for the stream's data error"""
+        out = []
+        for s in self.state():
+            code = s["status"] & 0xFF
+            out.append(None if code in (_lib.OK, _lib.E_NEED_INPUT) else
+                       _lib.lib().b200z_inflate_detail_message(s["status"]).decode())
+        return out
+
+    def set_dictionary(self, i, data):
+        """Inflater.SetDictionary on stream i; the next write() decodes what waited behind the header"""
+        a = np.ascontiguousarray(np.frombuffer(bytes(data), dtype=np.uint8))
+        _lib.raise_for(_lib.lib().b200z_inflate_streams_set_dictionary(self._h, i, a.ctypes.data if a.size else None, a.size))
+
+    def stats(self):
+        """{"runs": stream runs, "plans": plans run, "created": plans created, "held": most compressed bytes one stream
+        held at once, "workspace": most device workspace one plan took, "uploaded": host-to-device bytes of the runs}"""
+        v = np.zeros(6, dtype=np.int64)
+        _lib.raise_for(_lib.lib().b200z_inflate_streams_stats(self._h, v.ctypes.data, 6))
+        return dict(zip(("runs", "plans", "created", "held", "workspace", "uploaded"), (int(x) for x in v)))
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            try:
+                _lib.lib().b200z_inflate_streams_destroy(h)
+            except Exception:  # interpreter shutdown: the module globals may already be gone
+                pass
+
+    __del__ = close
+
 def deflate_batch(buffers, level=6, strategy=0, wrap=_lib.WRAP_RAW, end_mode=_lib.END_FINISH, devices=None):
     """Host buffers in, list of compressed bytes out (b200z_deflate_batch: H2D, kernels, D2H inside the call).
     devices: a list of CUDA device indices -- the batch is cut by bytes and every range runs on its own GPU at the same

@@ -79,16 +79,6 @@ std::string lzw_detail_msg(int32_t status, uint32_t value) {
 	return b;
 }
 
-// One run of a handle's single-stream plan on the legacy default stream; returns with the run's metadata in st.h and the
-// produced bytes in st.hout at the stream's out_off.  `in` is the handle's own pageable copy of the input.
-static int handle_run(b200z_plan *plan, Staging &st, const uint8_t *in, const uint32_t *check_seed) {
-	int rc = st.ensure(plan, false);
-	if (!rc) rc = stage_run(plan, st, &in, false, check_seed, 0, 0, nullptr);
-	if (rc) return rc;
-	B200Z_CUDA(cudaStreamSynchronize(0));
-	return streams_down(plan, st, nullptr, 0);
-}
-
 // =====================================================================================================
 // Deflater streams: the Deflater handle and the Deflater set share one host path
 // =====================================================================================================
@@ -580,18 +570,21 @@ static int set_runs(b200z_deflate_streams *S, const int32_t *op, const std::vect
 	return B200Z_OK;
 }
 
-// ---- Inflater handle ----------------------------------------------------------------------------------
+// ---- Inflater streams: the Inflater handle and the Inflater set share one host path ---------------------------------
 // The reference's Inflater is a mode machine that stops at any bit and resumes (Inflater.cs:73-86, :429-552).  The kernels
 // decode whole plans and report where a stream that ran out of input can be resumed (b200z_plan_get_resume_points): inside
-// a Huffman block at the first symbol not decoded, otherwise at the block header it stopped in.  Between SetInput calls the
-// handle keeps the window (the last 32 KiB of output), a copy of the current block's header when it stopped inside the
-// block, and the compressed bytes from the resume point on; the next run enters the block through the header copy
-// (b200z_inflate_plan_set_resume) and appends its output.  A stream stops inside a Huffman block only a symbol (at most 48
-// bits) short of the input's end, in a header at most a header (under 600 bytes) short, and in front of a stored block at
-// most 65535 + 5 bytes short: that, one header copy and the last SetInput are all the compressed bytes the handle holds,
-// whatever the block size, and no byte is decoded twice.
-struct InflaterH {
-	bool raw = false;
+// a Huffman block at the first symbol not decoded, otherwise at the block header it stopped in.  Between runs a stream
+// keeps its window (the last 32 KiB of output) in a device window pool, a copy of the current block's header when it
+// stopped inside the block, and the compressed bytes from the resume point on; the next run enters the block through the
+// header copy (b200z_inflate_plan_set_resume) and appends its output.  A stream stops inside a Huffman block only a symbol
+// (at most 48 bits) short of the input's end, in a header at most a header (under 600 bytes) short, and in front of a
+// stored block at most 65535 + 5 bytes short: that, one header copy and the last SetInput are all the compressed bytes a
+// stream holds, whatever the block size, and no byte is decoded twice.
+
+// What one Inflater stream carries between device runs, whoever drives it (a handle, or a stream of a set).
+struct InflateCarry {
+	int wrap = B200Z_WRAP_RAW; // RAW, ZLIB (Adler-32 and the zlib framing) or RAW_CRC32 (a CRC-32)
+	int32_t pool = 0;          // the stream's slot in its owner's window pool
 	std::vector<uint8_t> input; // compressed bytes from absolute offset in_base on (what lies in front of the resume point is dropped)
 	int64_t in_base = 0, in_total = 0; // in_total = bytes handed over since Reset = in_base + input.size()
 	bool new_input = false;
@@ -606,148 +599,455 @@ struct InflaterH {
 	int64_t rs_out = 0;        //   the block whose header `hdr` holds; output position there
 	std::vector<uint8_t> hdr;  // that block's header bytes, from bit hdr_sbit of hdr[0] on (empty: rs_bit is a header)
 	int32_t hdr_sbit = 0;
-	std::vector<uint8_t> window; // last <= 32768 bytes of (dictionary ++ output[0, rs_out)): OutputWindow's contents there
-	uint32_t run_adler = 1;    // Adler-32 of output[0, rs_out)
+	int32_t win_len = 0;       // last <= 32768 bytes of (dictionary ++ output[0, rs_out)), in the pool slot
+	uint32_t run_check = 1;    // Adler-32 / CRC-32 of output[0, rs_out)
 	std::vector<uint8_t> output; // decoded bytes from output position out_base on (delivered bytes in front of rs_out are dropped)
 	int64_t out_base = 0;
 	int64_t delivered = 0;
 	int64_t consumed = 0; // bytes of input the decoder has used (header + raw + trailer), absolute
-	uint32_t adler = 1;
-	int error = 0;
-	std::string error_msg;
-	int64_t stats[4] = {0, 0, 0, 0}; // b200z_inflater_get_stats
-	Staging st;
-	// one plan per handle, created for capacities and run below them (b200z_inflate_plan_set_lengths): a SetInput + Inflate
-	// pair costs the copies and the kernels, no allocation
-	b200z_plan *plan = nullptr;
-	int64_t plan_comp_cap = 0, plan_out_cap = 0;
-	~InflaterH() { b200z_plan_destroy(plan); }
+	uint32_t adler = 1;   // what Inflater.Adler reports (the handle)
+	int32_t error = 0;    // code | detail << 8 of the stream's data error
+	int64_t out_need = 0; // B200Z_E_NOMEM: the output capacity the next run asks for
+	int attempts = 0;     // runs in a row that ended in B200Z_E_NOMEM
+	int64_t decoded = 0;  // output bytes the runs produced (bytes decoded twice counted twice)
+	int64_t max_comp = 0, max_out = 0; // the most compressed / output bytes held at once
 	int64_t out_total() const { return out_base + (int64_t)output.size(); }
+	int ck_kind() const { return wrap == B200Z_WRAP_ZLIB ? 1 : (wrap == B200Z_WRAP_RAW_CRC32 ? 0 : -1); }
 	void note_held() {
-		stats[2] = std::max(stats[2], (int64_t)(input.size() + hdr.size()));
-		stats[3] = std::max(stats[3], (int64_t)(output.size() + window.size()));
+		max_comp = std::max(max_comp, (int64_t)(input.size() + hdr.size()));
+		max_out = std::max(max_out, (int64_t)output.size() + win_len);
+	}
+	void reset() { // (keeps wrap and pool)
+		const int w = wrap;
+		const int32_t p = pool;
+		*this = InflateCarry();
+		wrap = w;
+		pool = p;
+		run_check = w == B200Z_WRAP_RAW_CRC32 ? 0u : 1u; // Crc32.Reset / Adler32.Reset
 	}
 };
 
-// checksum and window advance over the next n bytes of output, which start at output position rs_out
-static int inflater_advance(InflaterH *d, int64_t n) {
-	const uint8_t *seg = d->output.data() + (d->rs_out - d->out_base);
-	if (!d->raw && n > 0) {
-		int rc = b200z_adler32(seg, n, &d->run_adler);
-		if (rc) return rc;
-	}
-	if (n >= 32768) d->window.assign(seg + n - 32768, seg + n);
-	else {
-		d->window.insert(d->window.end(), seg, seg + n);
-		if (d->window.size() > 32768) d->window.erase(d->window.begin(), d->window.end() - 32768);
-	}
-	d->rs_out += n;
-	return B200Z_OK;
+// What the runs of one owner (a handle, a set) share on the device: the window pool, the packed upload and the slot
+// descriptors, the staging of its plans, and what it counts.
+struct CarryDevice {
+	DevBuf pool, packed, slots;
+	Staging st;
+	int64_t h2d = 0;                     // host-to-device bytes the runs copied
+	int64_t plans_created = 0, workspace = 0;
+	int ensure_pool(int32_t n) { return pool.ensure((size_t)std::max<int32_t>(n, 1) * (size_t)kCarryWindow); }
+};
+
+// A raw inflate plan kept between runs, with the capacities it was created for (b200z_inflate_plan_set_lengths runs it
+// below them).
+struct CarryPlan {
+	b200z_plan *plan = nullptr;
+	std::vector<int64_t> comp_cap, out_cap;
+	CarryPlan() = default;
+	CarryPlan(CarryPlan &&o) noexcept : plan(o.plan), comp_cap(std::move(o.comp_cap)), out_cap(std::move(o.out_cap)) { o.plan = nullptr; }
+	CarryPlan(const CarryPlan &) = delete;
+	~CarryPlan() { b200z_plan_destroy(plan); }
+};
+
+// A run's compressed capacity: a power of two with room for the header copy and the bytes kept in front of a resume
+// point, so that equal pieces fit the plan their first run made.
+static int64_t carry_comp_cap(int64_t comp) {
+	int64_t cc = 65536;
+	while (cc < comp + 1024) cc *= 2;
+	return cc;
 }
+static int64_t carry_out_need(const InflateCarry *c, int64_t comp) { return std::max(c->out_need, comp * 8 + 65536); }
 
 // output in front of both the resume point and the delivery position is not needed any more.  Dropped once per run (a
 // reader has usually taken everything by then): erasing it on every Inflate() would move the rest of a run's output,
 // which can be 1032 times the input it came from, for every buffer handed out.
-static void inflater_trim_output(InflaterH *d) {
-	const int64_t keep_from = d->delivered < d->rs_out ? d->delivered : d->rs_out;
-	if (keep_from > d->out_base) {
-		d->output.erase(d->output.begin(), d->output.begin() + (keep_from - d->out_base));
-		d->out_base = keep_from;
+static void carry_trim_output(InflateCarry *c) {
+	const int64_t keep_from = c->delivered < c->rs_out ? c->delivered : c->rs_out;
+	if (keep_from > c->out_base) {
+		c->output.erase(c->output.begin(), c->output.begin() + (keep_from - c->out_base));
+		c->out_base = keep_from;
 	}
 }
 
-// decodes from the resume point to the end of what is available; appends to output, fills consumed / raw_done and moves
-// the resume point forward
-static int inflater_run_device(InflaterH *d) {
-	inflater_trim_output(d);
-	int64_t cap = 0;
-	for (int attempt = 0; attempt < 8; attempt++) {
-		// slot: window image, header copy, compressed bytes from the resume point's byte on
-		const int64_t tail_byte = d->rs_bit >> 3, slice_abs = d->raw_off + tail_byte;
-		const int64_t avail = d->in_total - slice_abs, H = (int64_t)d->hdr.size();
-		if (avail < 0 || slice_abs < d->in_base) {
+// The compressed bytes of a stream's next run: the header copy, then the input from the resume point's byte on.
+struct CarryCut {
+	int64_t tail_byte, slice_abs, avail, H, comp;
+};
+static CarryCut carry_cut(const InflateCarry *c) {
+	CarryCut u;
+	u.tail_byte = c->rs_bit >> 3;
+	u.slice_abs = c->raw_off + u.tail_byte;
+	u.avail = c->in_total - u.slice_abs;
+	u.H = (int64_t)c->hdr.size();
+	u.comp = u.H + u.avail;
+	return u;
+}
+
+// One device run of k streams as one raw inflate plan, on `cs`: each stream decodes from its resume point to the end of
+// what it holds, appends to its output, fills consumed / raw_done, and moves its resume point, window and running
+// checksum forward.  The run synchronises `cs` twice: once for the statuses and resume points, once for the output bytes
+// and checksums.  A stream whose output outgrew its capacity (B200Z_E_NOMEM) goes on from its resume point: it comes back
+// with out_need set for a later run.  A stream with corrupt data gets its error; the bytes in front of it are delivered.
+static int inflate_run(CarryDevice &dv, CarryPlan &cp, const std::vector<InflateCarry *> &s, cudaStream_t cs) {
+	const int k = (int)s.size();
+	std::vector<CarryCut> cut((size_t)k);
+	std::vector<int64_t> comp((size_t)k), D((size_t)k), skip((size_t)k), need((size_t)k);
+	std::vector<int32_t> sbit((size_t)k);
+	bool fits = cp.plan && cp.plan->n == k;
+	for (int i = 0; i < k; i++) {
+		InflateCarry *c = s[(size_t)i];
+		carry_trim_output(c);
+		const CarryCut &u = cut[(size_t)i] = carry_cut(c);
+		if (u.avail < 0 || u.slice_abs < c->in_base) {
 			set_error("inflater resume point outside the kept input");
 			return B200Z_E_INTERNAL;
 		}
-		const int64_t comp = H + avail, D = (int64_t)d->window.size();
-		const int32_t sbit = H ? d->hdr_sbit : (int32_t)(d->rs_bit & 7);
-		const int64_t skip = H ? 8 * H + (d->rs_bit & 7) : 0;
-		cap = std::max(cap, comp * 8 + 65536);
-		int rc;
-		if (!d->plan || comp > d->plan_comp_cap || cap > d->plan_out_cap) {
-			b200z_plan_destroy(d->plan);
-			d->plan = nullptr;
-			int64_t cc = 65536;
-			while (cc < comp) cc *= 2;
-			const int64_t oc = std::max(cap, cc * 8 + 65536), dc = 32768;
-			if ((rc = b200z_inflate_plan_create_ex(1, &cc, &oc, B200Z_WRAP_RAW, &dc, &d->plan))) return rc;
-			d->plan_comp_cap = cc;
-			d->plan_out_cap = oc;
+		comp[(size_t)i] = u.comp;
+		D[(size_t)i] = c->win_len;
+		sbit[(size_t)i] = u.H ? c->hdr_sbit : (int32_t)(c->rs_bit & 7);
+		skip[(size_t)i] = u.H ? 8 * u.H + (c->rs_bit & 7) : 0;
+		need[(size_t)i] = carry_out_need(c, u.comp);
+		if (fits && (u.comp > cp.comp_cap[(size_t)i] || need[(size_t)i] > cp.out_cap[(size_t)i])) fits = false;
+	}
+	int rc;
+	if (!fits) {
+		b200z_plan_destroy(cp.plan);
+		cp.plan = nullptr;
+		cp.comp_cap.resize((size_t)k);
+		cp.out_cap.resize((size_t)k);
+		for (int i = 0; i < k; i++) {
+			cp.comp_cap[(size_t)i] = carry_comp_cap(comp[(size_t)i]);
+			cp.out_cap[(size_t)i] = std::max(need[(size_t)i], cp.comp_cap[(size_t)i] * 8 + 65536);
 		}
-		b200z_plan *plan = d->plan;
-		if ((rc = b200z_inflate_plan_set_lengths(plan, &comp, &D))) return rc;
-		if ((rc = b200z_inflate_plan_set_resume(plan, &sbit, &skip))) return rc;
-		std::vector<uint8_t> slot;
-		slot.reserve((size_t)(D + comp));
-		slot.insert(slot.end(), d->window.begin(), d->window.end());
-		slot.insert(slot.end(), d->hdr.begin(), d->hdr.end());
-		const uint8_t *inp = d->input.data() + (slice_abs - d->in_base);
-		slot.insert(slot.end(), inp, inp + avail);
-		rc = handle_run(plan, d->st, slot.data(), nullptr);
-		const PipeMeta &r = d->st.h;
-		int64_t hb = 0, bb = 0, sb = 0, so = 0;
-		if (!rc) rc = b200z_plan_get_resume_points(plan, &hb, &bb, &sb, &so, nullptr);
+		const std::vector<int64_t> dc((size_t)k, kCarryWindow);
+		if ((rc = b200z_inflate_plan_create_ex(k, cp.comp_cap.data(), cp.out_cap.data(), B200Z_WRAP_RAW, dc.data(), &cp.plan))) return rc;
+		dv.plans_created++;
+		dv.workspace = std::max(dv.workspace, b200z_plan_workspace_bytes(cp.plan));
+	}
+	b200z_plan *plan = cp.plan;
+	if ((rc = b200z_inflate_plan_set_lengths(plan, comp.data(), D.data()))) return rc;
+	if ((rc = b200z_inflate_plan_set_resume(plan, sbit.data(), skip.data()))) return rc;
+	dv.h2d += 24ll * k; // (the lengths, start bits and jumps the two calls above write into the plan's workspace)
+	if ((rc = dv.st.ensure(plan, false))) return rc;
+	Staging &st = dv.st;
+	// one packed upload of every stream's header copy and compressed bytes; k_carry_stage puts them and the pool's windows
+	// into the slots
+	std::vector<CarrySlot> slot((size_t)k);
+	int64_t pk = 0;
+	for (int i = 0; i < k; i++) {
+		const InflateCarry *c = s[(size_t)i];
+		const CarryCut &u = cut[(size_t)i];
+		CarrySlot &sl = slot[(size_t)i];
+		sl.pk_off = pk;
+		sl.data_off = b200z_plan_data_offset(plan, i);
+		sl.comp = u.comp;
+		sl.out_off = plan->out_off[(size_t)i];
+		sl.out_pos = 0;
+		sl.pool = c->pool;
+		sl.win_len = c->win_len;
+		if (u.H) memcpy(st.hin.p + pk, c->hdr.data(), (size_t)u.H);
+		if (u.avail) memcpy(st.hin.p + pk + u.H, c->input.data() + (u.slice_abs - c->in_base), (size_t)u.avail);
+		pk = align_up(pk + u.comp, 16);
+	}
+	const size_t slot_bytes = sizeof(CarrySlot) * (size_t)k;
+	if ((rc = dv.packed.ensure((size_t)pk + 16)) || (rc = dv.slots.ensure(slot_bytes))) return rc;
+	if (pk) B200Z_CUDA(cudaMemcpyAsync(dv.packed.p, st.hin.p, (size_t)pk, cudaMemcpyHostToDevice, cs));
+	B200Z_CUDA(cudaMemcpyAsync(dv.slots.p, slot.data(), slot_bytes, cudaMemcpyHostToDevice, cs));
+	dv.h2d += pk + (int64_t)slot_bytes;
+	const CarrySlot *d_slots = reinterpret_cast<const CarrySlot *>(dv.slots.p);
+	if ((rc = carry_stage_launch(d_slots, k, dv.pool.p, dv.packed.p, st.din.p, cs))) return rc;
+	if ((rc = b200z_plan_run(plan, st.din.p, st.dout.p, st.d.out_len, st.d.status, st.d.check, st.d.in_used, cs))) return rc;
+	B200Z_CUDA(cudaMemcpyAsync(st.h.out_len, st.d.out_len, (size_t)k * (8 + 8 + 4 + 4), cudaMemcpyDeviceToHost, cs));
+	std::vector<int64_t> hb((size_t)k), bb((size_t)k), sb((size_t)k), so((size_t)k);
+	if ((rc = b200z_plan_get_resume_points(plan, hb.data(), bb.data(), sb.data(), so.data(), cs))) return rc; // (synchronises cs)
+	const PipeMeta &m = st.h;
+	// how far each stream's window and checksum move: all of a finished stream's output, up to the resume point otherwise
+	std::vector<int64_t> adv((size_t)k, 0), ck_off((size_t)k);
+	for (int i = 0; i < k; i++) {
+		const int code = m.status[i] & 0xFF;
+		const int64_t olen = m.out_len[i], H = cut[(size_t)i].H;
+		const int64_t sbi = sb[(size_t)i], soi = so[(size_t)i];
+		if (code == B200Z_OK) adv[(size_t)i] = olen;
+		else if (code == B200Z_E_NEED_INPUT || code == B200Z_E_NOMEM) {
+			if (soi < 0 || soi > olen || hb[(size_t)i] > bb[(size_t)i] || bb[(size_t)i] > sbi || sbi > 8 * comp[(size_t)i] || (sbi < 8 * H && soi != 0)) {
+				set_error("inflater resume point out of range");
+				return B200Z_E_INTERNAL;
+			}
+			if (sbi >= 8 * H) adv[(size_t)i] = soi; // (in front of that only when a run stopped before its first symbol)
+		}
+		slot[(size_t)i].out_pos = adv[(size_t)i];
+		ck_off[(size_t)i] = plan->out_off[(size_t)i];
+	}
+	B200Z_CUDA(cudaMemcpyAsync(dv.slots.p, slot.data(), slot_bytes, cudaMemcpyHostToDevice, cs));
+	dv.h2d += (int64_t)slot_bytes;
+	if ((rc = carry_window_launch(d_slots, k, st.din.p, st.dout.p, dv.pool.p, cs))) return rc;
+	for (int i = 0; i < k; i++)
+		if (m.out_len[i] > 0)
+			B200Z_CUDA(cudaMemcpyAsync(st.hout.p + plan->out_off[(size_t)i], st.dout.p + plan->out_off[(size_t)i], (size_t)m.out_len[i],
+			                           cudaMemcpyDeviceToHost, cs));
+	// the running checksums go on over the output the run left on the device; seeds and results live in the pinned
+	// metadata, which the device reads and writes in place (pinned memory is mapped under unified addressing)
+	const int kind = s[0]->ck_kind();
+	if (kind >= 0) {
+		for (int i = 0; i < k; i++) m.check[i] = s[(size_t)i]->run_check;
+		rc = b200z_checksum_batch_device(kind, st.dout.p, ck_off.data(), adv.data(), k, m.check, cs); // (synchronises cs)
+		dv.h2d += 16ll * k;
 		if (rc) return rc;
-		const int st = r.status[0] & 0xFF, detail = (r.status[0] >> 8) & 0xFF;
-		const int64_t olen = r.out_len[0];
-		d->stats[0]++;
-		d->stats[1] += olen;
+	} else {
+		B200Z_CUDA(cudaStreamSynchronize(cs));
+	}
+	for (int i = 0; i < k; i++) {
+		InflateCarry *c = s[(size_t)i];
+		const CarryCut &u = cut[(size_t)i];
+		const int code = m.status[i] & 0xFF;
+		const int64_t olen = m.out_len[i];
 		// this run's output is output[rs_out, rs_out + olen) (what it decoded in front of an error is delivered too)
-		const uint8_t *o = d->st.hout.p + plan->out_off[0];
-		d->output.resize((size_t)(d->rs_out - d->out_base));
-		d->output.insert(d->output.end(), o, o + olen);
-		if (st != B200Z_OK && st != B200Z_E_NEED_INPUT && st != B200Z_E_NOMEM) {
-			d->error = st;
-			d->error_msg = inflate_detail_msg(detail);
-			return B200Z_OK;
-		}
-		if (st == B200Z_OK) {
-			d->raw_done = true;
-			d->trailer_at = slice_abs + r.in_used[0] - H; // (the final block ends behind the header copy)
-			d->consumed = d->trailer_at;
-			return inflater_advance(d, olen);
-		}
-		if (so < 0 || so > olen || hb > bb || bb > sb || sb > 8 * comp || (sb < 8 * H && so != 0)) {
-			set_error("inflater resume point out of range");
-			return B200Z_E_INTERNAL;
-		}
-		if (sb >= 8 * H) { // (in front of that only when a run stopped before its first symbol)
-			if ((rc = inflater_advance(d, so))) return rc;
-			const uint8_t *c = slot.data() + D;
-			if (bb != hb) d->hdr.assign(c + (hb >> 3), c + ((bb + 7) >> 3)); // inside a Huffman block: keep its header
-			else d->hdr.clear();
-			d->hdr_sbit = (int32_t)(hb & 7);
-			d->rs_bit = 8 * tail_byte + (sb - 8 * H);
-		}
-		if (st == B200Z_E_NOMEM) {
-			cap = d->plan_out_cap * 8; // (the next attempt makes a larger plan and goes on from the resume point)
+		const uint8_t *o = st.hout.p + plan->out_off[(size_t)i];
+		c->output.resize((size_t)(c->rs_out - c->out_base));
+		c->output.insert(c->output.end(), o, o + olen);
+		c->decoded += olen;
+		c->out_need = 0;
+		if (code != B200Z_OK && code != B200Z_E_NEED_INPUT && code != B200Z_E_NOMEM) {
+			c->error = m.status[i];
+			c->attempts = 0;
 			continue;
 		}
-		d->consumed = d->in_total;
-		// compressed bytes in front of the resume point are never looked at again
-		const int64_t keep_from = d->raw_off + (d->rs_bit >> 3);
-		if (keep_from > d->in_base) {
-			d->input.erase(d->input.begin(), d->input.begin() + (keep_from - d->in_base));
-			d->in_base = keep_from;
+		const int64_t a = adv[(size_t)i];
+		if (kind >= 0) c->run_check = m.check[i];
+		c->win_len = (int32_t)std::min<int64_t>(kCarryWindow, c->win_len + a);
+		c->rs_out += a;
+		if (code == B200Z_OK) {
+			c->raw_done = true;
+			c->trailer_at = u.slice_abs + m.in_used[i] - u.H; // (the final block ends behind the header copy)
+			c->consumed = c->trailer_at;
+			c->attempts = 0;
+			continue;
 		}
-		return B200Z_OK;
+		const int64_t sbi = sb[(size_t)i];
+		if (sbi >= 8 * u.H) {
+			const uint8_t *p = st.hin.p + slot[(size_t)i].pk_off; // (the header copy, then the compressed bytes)
+			if (bb[(size_t)i] != hb[(size_t)i]) c->hdr.assign(p + (hb[(size_t)i] >> 3), p + ((bb[(size_t)i] + 7) >> 3)); // inside a Huffman block: keep its header
+			else c->hdr.clear();
+			c->hdr_sbit = (int32_t)(hb[(size_t)i] & 7);
+			c->rs_bit = 8 * u.tail_byte + (sbi - 8 * u.H);
+		}
+		if (code == B200Z_E_NOMEM) {
+			c->out_need = cp.out_cap[(size_t)i] * 8; // (the next run makes a larger plan and goes on from the resume point)
+			c->attempts++;
+			continue;
+		}
+		c->attempts = 0;
+		c->consumed = c->in_total;
+		// compressed bytes in front of the resume point are never looked at again
+		const int64_t keep_from = c->raw_off + (c->rs_bit >> 3);
+		if (keep_from > c->in_base) {
+			c->input.erase(c->input.begin(), c->input.begin() + (keep_from - c->in_base));
+			c->in_base = keep_from;
+		}
+	}
+	return B200Z_OK;
+}
+
+// A run takes a stream that has input it has not decoded, its zlib header read, no dictionary awaited, no error and
+// its final block not yet ended.  Only a stream whose last run ran out of output capacity goes on without new input.
+static bool carry_runs(const InflateCarry *c) { return !c->error && !c->need_dict && !c->raw_done && !c->finished; }
+
+// zlib: reads the header (Inflater.DecodeHeader :209-255) and the DICTID (DecodeDict :185-203) once their bytes are
+// there.  False while they are not, on an error and while a preset dictionary is awaited: the stream does not run.
+static bool carry_header(InflateCarry *c) {
+	if (c->wrap == B200Z_WRAP_ZLIB && !c->header_done) {
+		// (nothing is dropped from `input` before the header is done: in_base == 0 here)
+		if (c->input.size() < 2) {
+			c->consumed = (int64_t)c->input.size();
+			return false; // DecodeHeader needs 16 bits (Inflater.cs:209-215)
+		}
+		const int header = (c->input[0] << 8) | c->input[1];
+		if (header % 31 != 0) c->error = B200Z_E_DATA | 19 << 8;            // "Header checksum illegal"
+		else if ((header & 0x0f00) != (8 << 8)) c->error = B200Z_E_DATA | 20 << 8; // "Compression Method unknown"
+		if (c->error) return false;
+		if (header & 0x0020) {
+			// PRESET_DICT: DecodeDict reads the 4-byte DICTID MSB first (:185-203); Inflate() then returns 0 until
+			// SetDictionary supplies a dictionary with that Adler-32
+			if (c->input.size() < 6) {
+				c->consumed = (int64_t)c->input.size();
+				return false;
+			}
+			c->read_adler = ((uint32_t)c->input[2] << 24) | ((uint32_t)c->input[3] << 16) | ((uint32_t)c->input[4] << 8) | c->input[5];
+			c->need_dict = true;
+			c->adler = c->read_adler; // Inflater.Adler reports readAdler while the dictionary is awaited (:823-836)
+			c->header_done = true;
+			c->raw_off = 6;
+			c->consumed = 6;
+			c->new_input = true; // the bytes behind the DICTID wait for SetDictionary
+			return false;
+		}
+		c->header_done = true;
+		c->raw_off = 2;
+	}
+	if (c->need_dict) {
+		c->new_input = true;
+		return false;
+	}
+	return true;
+}
+
+// behind the final block: a zlib stream's Adler-32 trailer, read MSB first (DecodeChksum :397-418); until it is complete
+// only its bytes are awaited, the decoded output is all there
+static void carry_trailer(InflateCarry *c) {
+	if (!c->raw_done || c->finished) return;
+	if (c->wrap != B200Z_WRAP_ZLIB) {
+		c->finished = true;
+		return;
+	}
+	if (c->in_total - c->trailer_at < 4) {
+		c->consumed = c->in_total;
+		return;
+	}
+	const uint8_t *t = c->input.data() + (c->trailer_at - c->in_base);
+	const uint32_t want = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
+	c->adler = c->run_check; // of all the output
+	if (c->run_check != want) c->error = B200Z_E_DATA | 11 << 8; // "Adler chksum doesn't match"
+	c->consumed = c->trailer_at + 4;
+	c->finished = true;
+}
+
+// SetInput (the reference copies nothing; the carry keeps the bytes until they are decoded)
+static void carry_input(InflateCarry *c, const uint8_t *buf, int64_t len) {
+	if (c->finished) {
+		// after the end of the stream the reference keeps unread bytes as RemainingInput; replace them
+		c->input.resize((size_t)(c->consumed - c->in_base));
+		c->in_total = c->consumed;
+	}
+	c->input.insert(c->input.end(), buf, buf + len);
+	c->in_total += len;
+	c->new_input = true;
+	c->note_held();
+}
+
+// Inflater.SetDictionary :589-620: the dictionary's tail becomes the window in the stream's pool slot, the one time a
+// window crosses PCIe
+static int carry_set_dictionary(CarryDevice &dv, InflateCarry *c, const uint8_t *dict, int32_t len, cudaStream_t cs) {
+	if (len < 0 || (len > 0 && !dict)) {
+		set_error("buffer/count");
+		return B200Z_E_ARG;
+	}
+	if (!c->need_dict) {
+		set_error("Dictionary is not needed"); // InvalidOperationException
+		return B200Z_E_STATE;
+	}
+	uint32_t a = 1;
+	if (len > 0) {
+		int rc = b200z_adler32(dict, len, &a);
+		if (rc) return rc;
+	}
+	if (a != c->read_adler) {
+		set_error("Wrong adler checksum"); // SharpZipBaseException
+		return B200Z_E_DATA;
+	}
+	const int32_t keep = len > (int32_t)kCarryWindow ? (int32_t)kCarryWindow : len; // OutputWindow.CopyDict :160-166
+	if (keep > 0) {
+		B200Z_CUDA(cudaMemcpyAsync(dv.pool.p + ((int64_t)c->pool + 1) * kCarryWindow - keep, dict + (len - keep), (size_t)keep,
+		                           cudaMemcpyHostToDevice, cs));
+		B200Z_CUDA(cudaStreamSynchronize(cs));
+		dv.h2d += keep;
+	}
+	c->win_len = keep;
+	c->need_dict = false;
+	c->adler = 1;
+	c->new_input = true; // what was handed over behind the header can be decoded now
+	return B200Z_OK;
+}
+
+// The Inflater handle: one stream, one plan kept between runs, on the legacy default stream.
+struct InflaterH {
+	InflateCarry c;
+	CarryDevice dv;
+	CarryPlan cp;
+	int64_t runs = 0; // b200z_inflater_get_stats v[0]
+};
+
+// decodes from the resume point to the end of what is available, in runs of the handle's plan until no output capacity
+// is outgrown
+static int inflater_run_device(InflaterH *d) {
+	int rc = d->dv.ensure_pool(1);
+	if (rc) return rc;
+	const std::vector<InflateCarry *> one{&d->c};
+	for (int attempt = 0; attempt < 8; attempt++) {
+		if ((rc = inflate_run(d->dv, d->cp, one, 0))) return rc;
+		d->runs++;
+		if (d->c.out_need == 0) return B200Z_OK;
 	}
 	set_error("output larger than any capacity tried");
 	return B200Z_E_NOMEM;
 }
 
+// ---- Inflater set --------------------------------------------------------------------------------------------------
+// n Inflater streams of one wrap, driven together: a write appends every stream's piece (SetInput) and runs every stream
+// that can go on as plans on the set's CUDA stream.  Due streams are taken in order into plans of at most kInfPlanBytes
+// of compressed capacity and kInfPlanOut of output capacity (a stream larger than that runs alone), so one plan's device
+// workspace does not grow with the number of streams; the plans are kept and reused while the due streams fit them.
+// (The CPU test tier builds the kernels on the CUDA emulator with smaller values, for small data.)
+#ifndef B200Z_INFLATE_SET_PLAN_BYTES
+#define B200Z_INFLATE_SET_PLAN_BYTES (256ll << 20)
+#endif
+#ifndef B200Z_INFLATE_SET_PLAN_OUT
+#define B200Z_INFLATE_SET_PLAN_OUT (4ll << 30)
+#endif
+constexpr int64_t kInfPlanBytes = B200Z_INFLATE_SET_PLAN_BYTES;
+constexpr int64_t kInfPlanOut = B200Z_INFLATE_SET_PLAN_OUT;
 
 } // namespace b200z
+
+struct b200z_inflate_streams {
+	int device = -1, wrap = B200Z_WRAP_ZLIB;
+	std::vector<b200z::InflateCarry> s;
+	b200z::CarryDevice dv; // window pool of n slots; staging grows to the largest plan
+	std::vector<b200z::CarryPlan> plans; // the k-th plan of a round of runs
+	cudaStream_t cs = nullptr;
+	int broken = 0; // a run failed: the streams' state is not what their output says, no more writes
+	int64_t runs = 0, plans_run = 0; // b200z_inflate_streams_stats v[0], v[1]
+};
+
+namespace b200z {
+
+// runs every stream that can go on, in rounds: a stream whose output outgrew its capacity goes on in the next round
+static int inflate_set_runs(b200z_inflate_streams *S, std::vector<char> &due) {
+	const int n = (int)S->s.size();
+	for (int round = 0;; round++) {
+		std::vector<InflateCarry *> todo;
+		for (int i = 0; i < n; i++) {
+			InflateCarry *c = &S->s[(size_t)i];
+			if (!due[(size_t)i]) continue;
+			if (c->attempts >= 8) {
+				c->error = B200Z_E_NOMEM; // (output larger than any capacity tried)
+				c->attempts = 0;
+			}
+			if (carry_runs(c) && (round == 0 || c->out_need)) todo.push_back(c);
+		}
+		if (todo.empty()) return B200Z_OK;
+		size_t g = 0;
+		for (size_t a = 0; a < todo.size(); g++) {
+			std::vector<InflateCarry *> grp;
+			int64_t cb = 0, ob = 0;
+			for (; a < todo.size(); a++) {
+				const int64_t comp = carry_cut(todo[a]).comp, cc = carry_comp_cap(comp);
+				const int64_t oc = std::max(carry_out_need(todo[a], comp), cc * 8 + 65536);
+				if (!grp.empty() && (cb + cc > kInfPlanBytes || ob + oc > kInfPlanOut)) break;
+				cb += cc;
+				ob += oc;
+				grp.push_back(todo[a]);
+			}
+			if (S->plans.size() <= g) S->plans.emplace_back();
+			int rc = inflate_run(S->dv, S->plans[g], grp, S->cs);
+			if (rc) return rc;
+			S->runs += (int64_t)grp.size();
+			S->plans_run++;
+			for (InflateCarry *c : grp) c->note_held();
+		}
+	}
+}
+
+} // namespace b200z
+
 
 using namespace b200z;
 
@@ -955,7 +1255,7 @@ int b200z_inflater_create(int raw, void **h) {
 		return B200Z_E_ARG;
 	}
 	InflaterH *d = new InflaterH();
-	d->raw = raw != 0;
+	d->c.wrap = raw ? B200Z_WRAP_RAW : B200Z_WRAP_ZLIB;
 	*h = d;
 	return B200Z_OK;
 }
@@ -965,52 +1265,14 @@ int b200z_inflater_destroy(void *h) {
 }
 int b200z_inflater_reset(void *h) {
 	InflaterH *d = (InflaterH *)h;
-	d->input.clear();
-	d->output.clear();
-	d->window.clear();
-	d->new_input = d->finished = d->need_dict = d->header_done = d->raw_done = false;
-	d->in_base = d->in_total = 0;
-	d->trailer_at = 0;
-	d->raw_off = 0;
-	d->rs_bit = d->rs_out = 0;
-	d->hdr.clear();
-	d->hdr_sbit = 0;
-	for (int64_t &v : d->stats) v = 0;
-	d->run_adler = 1;
-	d->out_base = 0;
-	d->delivered = 0;
-	d->consumed = 0;
-	d->adler = 1;
-	d->error = 0;
-	d->read_adler = 0;
+	d->c.reset();
+	d->runs = 0;
 	return B200Z_OK;
 }
 int b200z_inflater_set_dictionary(void *h, const uint8_t *dict, int32_t len) {
 	InflaterH *d = (InflaterH *)h;
-	// Inflater.SetDictionary :589-620
-	if (len < 0 || (len > 0 && !dict)) {
-		set_error("buffer/count");
-		return B200Z_E_ARG;
-	}
-	if (!d->need_dict) {
-		set_error("Dictionary is not needed"); // InvalidOperationException
-		return B200Z_E_STATE;
-	}
-	uint32_t a = 1;
-	if (len > 0) {
-		int rc = b200z_adler32(dict, len, &a);
-		if (rc) return rc;
-	}
-	if (a != d->read_adler) {
-		set_error("Wrong adler checksum"); // SharpZipBaseException
-		return B200Z_E_DATA;
-	}
-	const int32_t keep = len > 32768 ? 32768 : len; // OutputWindow.CopyDict :160-166
-	d->window.assign(dict + (len - keep), dict + len);
-	d->need_dict = false;
-	d->adler = 1;
-	d->new_input = true; // what was handed over behind the header can be decoded now
-	return B200Z_OK;
+	int rc = d->c.need_dict ? d->dv.ensure_pool(1) : B200Z_OK;
+	return rc ? rc : carry_set_dictionary(d->dv, &d->c, dict, len, 0);
 }
 int b200z_inflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 	InflaterH *d = (InflaterH *)h;
@@ -1018,144 +1280,78 @@ int b200z_inflater_set_input(void *h, const uint8_t *buf, int32_t len) {
 		set_error("buffer/count");
 		return B200Z_E_ARG;
 	}
-	if (d->in_total > d->consumed && !d->finished) {
+	if (d->c.in_total > d->c.consumed && !d->c.finished) {
 		set_error("Old input was not completely processed"); // StreamManipulator.cs:263
 		return B200Z_E_STATE;
 	}
-	if (d->finished) {
-		// after the end of the stream the reference keeps unread bytes as RemainingInput; replace them
-		d->input.resize((size_t)(d->consumed - d->in_base));
-		d->in_total = d->consumed;
-	}
-	d->input.insert(d->input.end(), buf, buf + len);
-	d->in_total += len;
-	d->new_input = true;
-	d->note_held();
+	carry_input(&d->c, buf, len);
 	return B200Z_OK;
+}
+
+static int inflater_error(const InflateCarry &c) {
+	set_error("%s", inflate_detail_msg((c.error >> 8) & 0xFF));
+	return c.error & 0xFF;
 }
 
 int b200z_inflater_inflate(void *h, uint8_t *out, int32_t cap, int32_t *produced) {
 	InflaterH *d = (InflaterH *)h;
+	InflateCarry &c = d->c;
 	if (!produced || cap < 0 || (cap > 0 && !out)) {
 		set_error("bad arguments");
 		return B200Z_E_ARG;
 	}
 	*produced = 0;
-	if (d->error) {
-		set_error("%s", d->error_msg.c_str());
-		return d->error;
-	}
-	if (!d->finished && d->new_input) {
-		d->new_input = false;
-		if (!d->raw && !d->header_done) {
-			// (nothing is dropped from `input` before the header is done: in_base == 0 here)
-			if (d->input.size() < 2) {
-				d->consumed = (int64_t)d->input.size();
-				return B200Z_OK; // DecodeHeader needs 16 bits (Inflater.cs:209-215)
-			}
-			const int header = (d->input[0] << 8) | d->input[1];
-			if (header % 31 != 0) {
-				d->error = B200Z_E_DATA;
-				d->error_msg = "Header checksum illegal";
-			} else if ((header & 0x0f00) != (8 << 8)) {
-				d->error = B200Z_E_DATA;
-				d->error_msg = "Compression Method unknown";
-			}
-			if (d->error) {
-				set_error("%s", d->error_msg.c_str());
-				return d->error;
-			}
-			if (header & 0x0020) {
-				// PRESET_DICT: DecodeDict reads the 4-byte DICTID MSB first (:185-203); Inflate() then returns 0 until
-				// SetDictionary supplies a dictionary with that Adler-32
-				if (d->input.size() < 6) {
-					d->consumed = (int64_t)d->input.size();
-					return B200Z_OK;
-				}
-				d->read_adler = ((uint32_t)d->input[2] << 24) | ((uint32_t)d->input[3] << 16) | ((uint32_t)d->input[4] << 8) | d->input[5];
-				d->need_dict = true;
-				d->adler = d->read_adler; // Inflater.Adler reports readAdler while the dictionary is awaited (:823-836)
-				d->header_done = true;
-				d->raw_off = 6;
-				d->consumed = 6;
-				d->new_input = true; // the bytes behind the DICTID wait for SetDictionary
-				return B200Z_OK;
-			}
-			d->header_done = true;
-			d->raw_off = 2;
-		}
-		if (d->need_dict) {
-			d->new_input = true;
-			return B200Z_OK;
-		}
-		if (!d->raw_done) {
+	if (c.error) return inflater_error(c);
+	if (!c.finished && c.new_input) {
+		c.new_input = false;
+		if (!carry_header(&c)) return c.error ? inflater_error(c) : B200Z_OK;
+		if (!c.raw_done) {
 			int rc = inflater_run_device(d);
-			d->note_held();
+			c.note_held();
 			if (rc) return rc;
 		}
-		if (d->raw_done && d->raw) {
-			d->finished = true;
-		} else if (d->raw_done) {
-			// Adler32 trailer, read MSB first (DecodeChksum :397-418); until it is complete only its bytes are awaited, the
-			// decoded output is all there
-			if (d->in_total - d->trailer_at < 4) {
-				d->consumed = d->in_total;
-			} else {
-				const uint8_t *t = d->input.data() + (d->trailer_at - d->in_base);
-				const uint32_t want = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
-				d->adler = d->run_adler; // of all the output
-				if (d->run_adler != want) {
-					d->error = B200Z_E_DATA;
-					d->error_msg = "Adler chksum doesn't match";
-				}
-				d->consumed = d->trailer_at + 4;
-				d->finished = true;
-			}
-		}
+		carry_trailer(&c);
 	}
-	size_t avail = (size_t)(d->out_total() - d->delivered);
+	size_t avail = (size_t)(c.out_total() - c.delivered);
 	size_t take = avail < (size_t)cap ? avail : (size_t)cap;
-	if (take) memcpy(out, d->output.data() + (d->delivered - d->out_base), take);
-	d->delivered += (int64_t)take;
+	if (take) memcpy(out, c.output.data() + (c.delivered - c.out_base), take);
+	c.delivered += (int64_t)take;
 	*produced = (int32_t)take;
-	if (take == 0 && d->error) {
-		set_error("%s", d->error_msg.c_str());
-		return d->error;
-	}
+	if (take == 0 && c.error) return inflater_error(c);
 	return B200Z_OK;
 }
 int b200z_inflater_needs_input(void *h, int *flag) {
 	InflaterH *d = (InflaterH *)h;
-	*flag = (d->in_total <= d->consumed) ? 1 : 0; // StreamManipulator.IsNeedingInput
+	*flag = (d->c.in_total <= d->c.consumed) ? 1 : 0; // StreamManipulator.IsNeedingInput
 	return B200Z_OK;
 }
 int b200z_inflater_needs_dictionary(void *h, int *flag) {
-	*flag = ((InflaterH *)h)->need_dict ? 1 : 0; // mode == DECODE_DICT && neededBits == 0 (Inflater.cs:792-798)
+	*flag = ((InflaterH *)h)->c.need_dict ? 1 : 0; // mode == DECODE_DICT && neededBits == 0 (Inflater.cs:792-798)
 	return B200Z_OK;
 }
 int b200z_inflater_is_finished(void *h, int *flag) {
-	InflaterH *d = (InflaterH *)h;
+	const InflateCarry &c = ((InflaterH *)h)->c;
 	// Inflater.cs:806-812; a trailer that did not verify is an exception from Inflate() in the reference (DecodeChksum
 	// :397-418), so the stream is not "finished" as long as that error has not been delivered
-	*flag = (d->finished && !d->error && d->delivered == d->out_total()) ? 1 : 0;
+	*flag = (c.finished && !c.error && c.delivered == c.out_total()) ? 1 : 0;
 	return B200Z_OK;
 }
 int b200z_inflater_remaining_input(void *h, int32_t *v) {
-	InflaterH *d = (InflaterH *)h;
-	*v = (int32_t)(d->in_total - d->consumed);
+	const InflateCarry &c = ((InflaterH *)h)->c;
+	*v = (int32_t)(c.in_total - c.consumed);
 	return B200Z_OK;
 }
 int b200z_inflater_total_in(void *h, int64_t *v) {
-	*v = ((InflaterH *)h)->consumed; // totalIn - RemainingInput (Inflater.cs:862-868)
+	*v = ((InflaterH *)h)->c.consumed; // totalIn - RemainingInput (Inflater.cs:862-868)
 	return B200Z_OK;
 }
 int b200z_inflater_total_out(void *h, int64_t *v) {
-	*v = ((InflaterH *)h)->delivered;
+	*v = ((InflaterH *)h)->c.delivered;
 	return B200Z_OK;
 }
 int b200z_inflater_adler(void *h, uint32_t *v) {
-	InflaterH *d = (InflaterH *)h;
-	*v = d->raw ? 0u : d->adler;
+	const InflateCarry &c = ((InflaterH *)h)->c;
+	*v = c.wrap == B200Z_WRAP_RAW ? 0u : c.adler;
 	return B200Z_OK;
 }
 int b200z_inflater_get_stats(void *h, int64_t *v, int32_t cap) {
@@ -1164,7 +1360,8 @@ int b200z_inflater_get_stats(void *h, int64_t *v, int32_t cap) {
 		return B200Z_E_ARG;
 	}
 	const InflaterH *d = (const InflaterH *)h;
-	for (int32_t i = 0; i < cap && i < 4; i++) v[i] = d->stats[i];
+	const int64_t s[4] = {d->runs, d->c.decoded, d->c.max_comp, d->c.max_out};
+	for (int32_t i = 0; i < cap && i < 4; i++) v[i] = s[i];
 	return B200Z_OK;
 }
 
@@ -1298,5 +1495,175 @@ int b200z_deflate_streams_destroy(b200z_deflate_streams *S) {
 	delete S;
 	return B200Z_OK;
 }
+
+int b200z_inflate_streams_create(int32_t n, int wrap, b200z_inflate_streams **s) {
+	if (!s || n < 0) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	if (wrap != B200Z_WRAP_RAW && wrap != B200Z_WRAP_ZLIB && wrap != B200Z_WRAP_RAW_CRC32) {
+		set_error("wrap: RAW, ZLIB or RAW_CRC32");
+		return B200Z_E_ARG;
+	}
+	int rc = ensure_init();
+	if (rc) return rc;
+	b200z_inflate_streams *S = new b200z_inflate_streams();
+	S->device = current_device();
+	DeviceGuard guard(S->device);
+	S->wrap = wrap;
+	S->s = std::vector<InflateCarry>((size_t)n);
+	for (int32_t i = 0; i < n; i++) {
+		InflateCarry &c = S->s[(size_t)i];
+		c.wrap = wrap;
+		c.pool = i;
+		c.reset();
+	}
+	if ((rc = S->dv.ensure_pool(n))) {
+		delete S;
+		return rc;
+	}
+	if (cudaStreamCreateWithFlags(&S->cs, cudaStreamNonBlocking) != cudaSuccess) {
+		delete S;
+		set_error("cudaStreamCreate failed");
+		return B200Z_E_CUDA;
+	}
+	*s = S;
+	return B200Z_OK;
+}
+
+// a stream's status as a write reports it: its data error, B200Z_E_NEED_INPUT while it is not finished, B200Z_OK after
+static int32_t inflate_set_status(const InflateCarry &c) { return c.error ? c.error : (c.finished ? B200Z_OK : B200Z_E_NEED_INPUT); }
+
+int b200z_inflate_streams_write(b200z_inflate_streams *S, const uint8_t *const *in, const int64_t *len, int32_t *status) {
+	if (!S || (!S->s.empty() && (!in || !len || !status))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	const int n = (int)S->s.size();
+	for (int i = 0; i < n; i++) // (nothing is taken when an argument is bad)
+		if (len[i] < 0 || len[i] > 0x7FFFFFFF || (len[i] > 0 && !in[i])) {
+			set_error("stream %d: buffer/count", i);
+			return B200Z_E_ARG;
+		}
+	if (S->broken) {
+		set_error("an earlier run of this Inflater set failed with status %d", S->broken);
+		return S->broken;
+	}
+	DeviceGuard guard(S->device);
+	std::vector<char> due((size_t)n, 0), late((size_t)n, 0);
+	for (int i = 0; i < n; i++) {
+		InflateCarry &c = S->s[(size_t)i];
+		if (len[i] > 0) {
+			if (c.finished) late[(size_t)i] = 1; // "Finish() already called" in the Deflater set: the input is refused
+			else if (!c.error) carry_input(&c, in[i], len[i]);
+		}
+		if (!c.finished && !c.error && c.new_input) {
+			c.new_input = false;
+			due[(size_t)i] = carry_header(&c) ? 1 : 0;
+		}
+	}
+	const int rc = inflate_set_runs(S, due);
+	if (rc) {
+		S->broken = rc;
+		return rc;
+	}
+	int first = -1;
+	for (int i = 0; i < n; i++) {
+		InflateCarry &c = S->s[(size_t)i];
+		if (due[(size_t)i]) carry_trailer(&c);
+		c.note_held();
+		status[i] = late[(size_t)i] ? B200Z_E_STATE : inflate_set_status(c);
+		if (first < 0 && status[i] != B200Z_OK && (status[i] & 0xFF) != B200Z_E_NEED_INPUT) first = i;
+	}
+	if (first < 0) return B200Z_OK;
+	if (late[(size_t)first]) set_error("stream %d: input behind the end of the stream", first);
+	else set_error("stream %d: %s", first, inflate_detail_msg((status[first] >> 8) & 0xFF));
+	return status[first] & 0xFF;
+}
+
+int b200z_inflate_streams_read(b200z_inflate_streams *S, uint8_t *const *out, const int64_t *cap, int64_t *got) {
+	if (!S || (!S->s.empty() && (!out || !cap || !got))) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	const int n = (int)S->s.size();
+	for (int i = 0; i < n; i++)
+		if (cap[i] < 0 || (cap[i] > 0 && !out[i])) {
+			set_error("stream %d: buffer/count", i);
+			return B200Z_E_ARG;
+		}
+	for (int i = 0; i < n; i++) {
+		InflateCarry &c = S->s[(size_t)i];
+		const int64_t take = std::min<int64_t>(cap[i], c.out_total() - c.delivered);
+		if (take > 0) memcpy(out[i], c.output.data() + (c.delivered - c.out_base), (size_t)take);
+		c.delivered += take;
+		got[i] = take;
+	}
+	return B200Z_OK;
+}
+
+int b200z_inflate_streams_state(b200z_inflate_streams *S, int32_t *flags, int64_t *total_in, int64_t *total_out, int64_t *remaining,
+                                int32_t *status) {
+	if (!S) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	for (size_t i = 0; i < S->s.size(); i++) {
+		const InflateCarry &c = S->s[i];
+		if (flags) flags[i] = (c.finished && !c.error ? 1 : 0) | (c.need_dict ? 2 : 0);
+		if (total_in) total_in[i] = c.consumed;
+		if (total_out) total_out[i] = c.out_total();
+		if (remaining) remaining[i] = c.in_total - c.consumed;
+		if (status) status[i] = inflate_set_status(c);
+	}
+	return B200Z_OK;
+}
+
+int b200z_inflate_streams_check(b200z_inflate_streams *S, uint32_t *check) {
+	if (!S || (!S->s.empty() && !check)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	for (size_t i = 0; i < S->s.size(); i++) {
+		const InflateCarry &c = S->s[i];
+		check[i] = S->wrap == B200Z_WRAP_RAW ? 0u : (c.need_dict ? c.read_adler : c.run_check);
+	}
+	return B200Z_OK;
+}
+
+int b200z_inflate_streams_set_dictionary(b200z_inflate_streams *S, int32_t i, const uint8_t *dict, int32_t len) {
+	if (!S || i < 0 || i >= (int32_t)S->s.size()) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	DeviceGuard guard(S->device);
+	return carry_set_dictionary(S->dv, &S->s[(size_t)i], dict, len, S->cs);
+}
+
+int b200z_inflate_streams_stats(b200z_inflate_streams *S, int64_t *v, int32_t cap) {
+	if (!S || cap < 0 || (cap > 0 && !v)) {
+		set_error("bad arguments");
+		return B200Z_E_ARG;
+	}
+	int64_t held = 0;
+	for (const InflateCarry &c : S->s) held = std::max(held, c.max_comp);
+	const int64_t s[6] = {S->runs, S->plans_run, S->dv.plans_created, held, S->dv.workspace, S->dv.h2d};
+	for (int32_t i = 0; i < cap && i < 6; i++) v[i] = s[i];
+	return B200Z_OK;
+}
+
+int b200z_inflate_streams_destroy(b200z_inflate_streams *S) {
+	if (!S) return B200Z_OK;
+	DeviceGuard guard(S->device); // (the device buffers and plans go while the set's device is current)
+	if (S->cs) {
+		cudaStreamSynchronize(S->cs);
+		cudaStreamDestroy(S->cs);
+	}
+	delete S;
+	return B200Z_OK;
+}
+
+const char *b200z_inflate_detail_message(int32_t status) { return inflate_detail_msg((status >> 8) & 0xFF); }
+
 
 } // extern "C"

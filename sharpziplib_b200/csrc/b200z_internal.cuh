@@ -226,4 +226,15 @@ int lzw_plan_create(int32_t n, const int64_t *comp_len, const int64_t *out_cap, 
 int lzw_plan_run(b200z_plan *p, const uint8_t *d_in, uint8_t *d_out, int64_t *d_out_len, int32_t *d_status, uint32_t *d_value,
                  int64_t *d_in_used, cudaStream_t s);
 int lzw_plan_stats(b200z_plan *p, uint32_t *v, int32_t cap, cudaStream_t s);
+// b200z_inflate_streams.cu: the window pool of the inflate carry.  Pool slot p is kCarryWindow bytes; its window is the
+// slot's last win_len bytes.  Per stream of a run: the packed upload holds comp bytes (header copy, then compressed bytes)
+// at pk_off; the plan's compressed bytes start at data_off of the input blob, the window in front of them; out_pos is the
+// output the window moves over after the run (k_carry_window).
+constexpr int64_t kCarryWindow = 32768;
+struct CarrySlot {
+	int64_t pk_off, data_off, comp, out_off, out_pos;
+	int32_t pool, win_len;
+};
+int carry_stage_launch(const CarrySlot *d_slots, int32_t k, uint8_t *d_pool, const uint8_t *d_packed, uint8_t *d_in, cudaStream_t s);
+int carry_window_launch(const CarrySlot *d_slots, int32_t k, const uint8_t *d_in, const uint8_t *d_out, uint8_t *d_pool, cudaStream_t s);
 } // namespace b200z
